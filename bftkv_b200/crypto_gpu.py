@@ -25,8 +25,9 @@ ErrInvalidTransportSecurityData = "crypto: invalid transport security data"
 ErrMessageBody = "message body / nonce error"
 ErrMessageUnsupported = "unsupported message form (compressed data)"
 ErrNotBuilt = "gpu: key size / curve not built into libbftq (the shim re-runs the item on crypto/pgp)"
+ErrMDC = "openpgp: invalid signature: hash mismatch"        # seMDCReader.Close's SignatureError, returned by ReadAll as is
 _ERR = {0: None, -6: ErrInvalidSignature, -7: ErrInsufficientNumberOfSignatures, -8: ErrDecryptionFailed, -9: ErrInvalidTransportSecurityData,
-        -10: ErrMessageBody, -11: ErrMessageUnsupported}
+        -10: ErrMessageBody, -11: ErrMessageUnsupported, -12: ErrMDC}
 _ERR_SIG = dict(_ERR)
 _ERR_SIG[-11] = ErrNotBuilt
 
@@ -101,6 +102,15 @@ class Keyring:
         buf = np.frombuffer(key_blocks or b"\0", np.uint8).copy()
         n = C.c_uint32()
         _lib.check(self._lib.bftq_keyring_add(self._h, C.c_void_p(buf.ctypes.data), len(key_blocks), int(priv), C.byref(n)))
+        return n.value
+
+    def register_private(self, packets: bytes) -> int:
+        """bftq_keyring_add_private: OpenPGP secret-key packets (unprotected RSA-2048) -> keys registered on the device."""
+        buf = np.frombuffer(packets or b"\0", np.uint8).copy()
+        n = C.c_uint32()
+        rc = self._lib.bftq_keyring_add_private(self._h, C.c_void_p(buf.ctypes.data), len(packets), C.byref(n))
+        buf[:] = 0
+        _lib.check(rc)
         return n.value
 
     def remove(self, ids: Sequence[int]):
@@ -322,6 +332,31 @@ class Message:
 
     def decrypt_verify(self, stream: bytes):
         return self.decrypt_verify_batch([stream])[0]
+
+    def decrypt_batch(self, raws: Sequence[bytes]):
+        """PGPMessage.Decrypt on raw encrypted transport messages (bftq_message_decrypt_batch): the session key is recovered
+        with the private key registered by Keyring.register_private.  -> list of dicts as decrypt_verify_batch, plus
+        "code" (the BFTQ_ERR_* value)."""
+        n = len(raws)
+        if n == 0:
+            return []
+        blob, off = _blob(raws)
+        total = int(off[-1])
+        err = np.zeros(n, np.int32)
+        by = np.zeros(n, np.uint64)
+        flags = np.zeros(n, np.uint8)
+        plain, nonce = np.zeros(max(total, 1), np.uint8), np.zeros(max(total, 1), np.uint8)
+        plen, nlen = np.zeros(n, np.uint32), np.zeros(n, np.uint32)
+        p = lambda a: C.c_void_p(a.ctypes.data)
+        _lib.check(self.kr._lib.bftq_message_decrypt_batch(self.kr._h, p(blob), p(off), n, p(err), p(by), p(flags), p(plain), p(plen), p(nonce), p(nlen)))
+        out = []
+        for i in range(n):
+            o = int(off[i])
+            ok_body = int(err[i]) in (0, -6)
+            out.append({"code": int(err[i]), "err": _ERR[int(err[i])], "plain": bytes(plain[o:o + int(plen[i])]) if ok_body else None,
+                        "nonce": bytes(nonce[o:o + int(nlen[i])]) if ok_body else None, "signed_by_key_id": int(by[i]),
+                        "signer_known": bool(flags[i] & 1), "binary": bool(flags[i] & 2)})
+        return out
 
 
 def read_responses_batch(kr: "Keyring", qcs, op_off, peer_ids, msgs: Sequence[bytes], nonces, pre_status=None, blobs=None):

@@ -13,6 +13,7 @@
 #include "pgp_digest.cuh"
 #include "pgp_parse.cuh"
 #include "msg_parse.cuh"
+#include "msg_decrypt.cuh"
 #include "pgp_host.hpp"
 #include "wotqs_host.hpp"
 
@@ -228,7 +229,11 @@ struct bftq_engine {
   uint32_t packer_flags = 0;   // BFTQ_F_* the packet-level entry points pass to K1 (bftq_engine_set_verify_flags / env BFTQ_STRICT_RANGE)
   int rsa_t = 4;          // lanes per signature (env BFTQ_RSA_T)
   int rsa_block = 128;
+  std::mutex kr_mu;
+  std::vector<bftq_keyring*> keyrings;           // live keyrings: their private-key tables are zeroed at shutdown
 };
+void priv_release(bftq_keyring* kr);             // decrypt_host.inc: zero and free a keyring's private-key table
+void keyring_detach(bftq_keyring* kr);           // a keyring that outlives its engine becomes parse-only
 
 namespace {
 
@@ -695,6 +700,11 @@ int bftq_bind_thread(bftq_engine* e) {
 void bftq_shutdown(bftq_engine* e) {
   if (!e) return;
   cudaSetDevice(e->device);
+  {
+    std::lock_guard<std::mutex> g(e->kr_mu);
+    for (bftq_keyring* kr : e->keyrings) { priv_release(kr); keyring_detach(kr); }
+    e->keyrings.clear();
+  }
   for (auto& kv : e->host_allocs) cudaFreeHost(kv.first);
   for (auto* s : e->slots) {
     if (s->stream) { cudaStreamSynchronize(s->stream); cudaStreamDestroy(s->stream); }
@@ -1767,6 +1777,7 @@ int bftq_pgp_digest_batch(bftq_engine* e, const uint8_t* data_blob, const uint64
 // ---- host packer ------------------------------------------------------------------------------
 }  // extern "C"
 #include "packer_host.inc"
+#include "decrypt_host.inc"
 
 // ---- quorum-descriptor builder ------------------------------------------------------------------
 // The descriptor the reference recomputes on EVERY call (client.go:64,101,141,238; server.go:182,211,237,300,473) is a

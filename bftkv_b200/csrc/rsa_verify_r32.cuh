@@ -156,7 +156,8 @@ __device__ __forceinline__ uint32_t lane_carry_in(const uint32_t gbits, const ui
 
 // The tail of a Montgomery product: merges the E / O accumulators and the pending carries into W limbs per lane,
 // resolves the carries across the four lanes and subtracts n once when the result overflowed 2^(128 W).
-template <int W>
+// CT: the subtraction is always computed and selected with a mask (no branch on the data: K6a, msg_decrypt.cuh).
+template <int W, bool CT = false>
 __device__ __forceinline__ void mont_finish(uint32_t (&out)[W], Acc<W>& A, const uint32_t cin, const uint32_t Z, const uint32_t (&n)[W],
                                             const int r, const int gbase) {
   // ---- merge E, O and the pending carry into 16 limbs + overflow ------------------------------
@@ -180,7 +181,7 @@ __device__ __forceinline__ void mont_finish(uint32_t (&out)[W], Acc<W>& A, const
   const uint32_t top_hi = __shfl_sync(kFull, hi, gbase + T - 1);
   const bool overflow = (top_hi + ctop) != 0u;          // result >= 2^2048: subtract n once
   // ---- conditional subtraction ---------------------------------------------------------------
-  if (__any_sync(kFull, overflow)) {
+  if (CT || __any_sync(kFull, overflow)) {
     uint32_t d[W];
     const uint32_t bo = sub_n(d, v, n);
     bool zeros = true;
@@ -191,7 +192,11 @@ __device__ __forceinline__ void mont_finish(uint32_t (&out)[W], Acc<W>& A, const
     uint32_t btop;
     const uint32_t bi = lane_carry_in(bgb, bpb, r, btop);
     ripple_sub(d, bi);
-    if (overflow) {
+    if (CT) {
+      const uint32_t m = 0u - (uint32_t)overflow;
+#pragma unroll
+      for (int k = 0; k < W; k++) v[k] = (d[k] & m) | (v[k] & ~m);
+    } else if (overflow) {
 #pragma unroll
       for (int k = 0; k < W; k++) v[k] = d[k];
     }
@@ -202,7 +207,7 @@ __device__ __forceinline__ void mont_finish(uint32_t (&out)[W], Acc<W>& A, const
 
 // out = a * b * R^-1 mod n with R = 2^(128 W), out < R ("almost Montgomery").  a, b < R as W limbs/lane.
 // All 32 lanes of the warp must call this together.
-template <int W, bool STEP_SYNC = false>
+template <int W, bool STEP_SYNC = false, bool CT = false>
 __device__ __forceinline__ void mont_mul(uint32_t (&out)[W], const uint32_t (&a)[W], const uint32_t (&b)[W],
                                          const uint32_t (&n)[W], const uint32_t n0inv, const int r, const int gbase) {
   Acc<W> A;
@@ -260,7 +265,7 @@ __device__ __forceinline__ void mont_mul(uint32_t (&out)[W], const uint32_t (&a)
                    : "+r"(A.E[W - 2]), "+r"(A.E[W - 1]), "+r"(A.E[W]), "+r"(A.E[W + 1]) : "r"(r0), "r"(r1));
     }
   }
-  mont_finish(out, A, cin, Z, n, r, gbase);
+  mont_finish<W, CT>(out, A, cin, Z, n, r, gbase);
 }
 
 // x >= n ?  (lane-distributed compare)

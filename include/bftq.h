@@ -46,6 +46,7 @@ extern "C" {
 #define BFTQ_ERR_NOT_SIGNED        -9   /* crypto.ErrInvalidTransportSecurityData (crypto_pgp.go:458-460)  */
 #define BFTQ_ERR_MESSAGE_BODY     -10   /* the literal body ends early / FileName is not base64: Decrypt returns that error as is */
 #define BFTQ_ERR_UNSUPPORTED      -11   /* a form the reference's library handles and this build does not (compressed data)       */
+#define BFTQ_ERR_MDC             -12   /* the SEIPD packet's modification detection code does not match: ReadAll's error, returned as is */
 
 /* ---- per-item status bytes (SURVEY §8b "Errors") --------------------------------------------
  * The reference collapses every failure to ErrInvalidSignature (crypto_pgp.go:325-327); the shim
@@ -407,6 +408,32 @@ int bftq_signature_signers(bftq_keyring* kr, const uint8_t* sig, uint64_t sig_le
 int bftq_message_verify_batch(bftq_keyring* kr, const uint8_t* msg_blob, const uint64_t* msg_off, uint64_t n_items, int32_t* out_err,
                               uint64_t* out_signed_by, uint8_t* out_flags, uint8_t* out_plain_blob, uint32_t* out_plain_len,
                               uint8_t* out_nonce_blob, uint32_t* out_nonce_len);
+
+/* ---- the encryption layer (K6): opt-in private keys on the device --------------------------------------------------
+ * Registers the private halves of RSA keys for decryption: a stream of OpenPGP secret-key packets (tag 5 / 7, v4, S2K usage
+ * 0), as gpg --export-secret-keys writes them for an unprotected key, or as x/crypto's packet.PrivateKey.Serialize writes the
+ * entity's primary key and each subkey.  Keys are matched by key id (fingerprint of the public part); an entity registered
+ * with bftq_keyring_add(priv = 1) uses them.  Nothing secret reaches the device unless it is registered here.  Each key is
+ * checked (2-byte checksum, p q == n, n of exactly 2048 bits with 1024-bit p and q) and must pass one encrypt / decrypt round
+ * trip on the device.  Keys that fail are not registered: BFTQ_ERR_UNSUPPORTED_KEY (protected, not RSA, other sizes,
+ * inconsistent) or BFTQ_ERR_MALFORMED (framing, checksum) is returned after the other keys of the stream were processed;
+ * *n_keys = keys registered.  The private halves live in one device allocation per keyring, zeroed before it is freed
+ * (bftq_keyring_remove of the owning entity, bftq_keyring_destroy); host copies are wiped after upload. */
+int bftq_keyring_add_private(bftq_keyring* kr, const uint8_t* packets, uint64_t len, uint32_t* n_keys);
+
+/* The whole of PGPMessage.Decrypt (crypto_pgp.go:453-471) on raw transport messages: openpgp.ReadMessage's PKESK loop
+ * (each PKESK in order, KeysById over secring ++ keyring, keys without a private half skipped), the RSA-CRT session-key
+ * recovery (K6a), the quick check of each candidate in order and the AES-CFB / SHA-1 MDC layer (K6b), then the signature
+ * half of bftq_message_verify_batch on the decrypted packet stream.  Outputs as bftq_message_verify_batch, at raw_off.
+ *   out_err[i]  0 | BFTQ_ERR_INVALID_SIGNATURE | BFTQ_ERR_MALFORMED (ReadMessage failed: no key decrypts, bad framing, unknown
+ *               cipher, wrong key length, a session-key message shorter than 3 bytes — where the reference panics) |
+ *               BFTQ_ERR_NOT_SIGNED (also: the message is not encrypted) | BFTQ_ERR_MESSAGE_BODY | BFTQ_ERR_MDC |
+ *               BFTQ_ERR_UNSUPPORTED: the shim re-runs the item on crypto/pgp — compressed inner streams, CAST5 / 3DES,
+ *               tag 9 without MDC, tag 3, ElGamal PKESKs, wildcard key id 0, a secring key without a registered private half,
+ *               several private candidates for one PKESK, packets behind the encrypted packet. */
+int bftq_message_decrypt_batch(bftq_keyring* kr, const uint8_t* raw_blob, const uint64_t* raw_off, uint64_t n_items, int32_t* out_err,
+                               uint64_t* out_signed_by, uint8_t* out_flags, uint8_t* out_plain_blob, uint32_t* out_plain_len,
+                               uint8_t* out_nonce_blob, uint32_t* out_nonce_len);
 
 /* Batching aggregator: bftkv calls Signature.Verify one (tbs, sig) at a time from many goroutines
  * (one per peer in transport.Multicast, transport/transport.go:110-127; one per HTTP request on the
