@@ -16,6 +16,7 @@
 #include "msg_decrypt.cuh"
 #include "pgp_host.hpp"
 #include "wotqs_host.hpp"
+#include "bignum_host.hpp"
 
 #include <algorithm>
 #include <array>
@@ -53,40 +54,8 @@ int fail(int code, const std::string& msg) {
       return fail(BFTQ_ERR_CUDA, std::string(#call) + ": " + cudaGetErrorString(_e));         \
   } while (0)
 
-// ---- tiny host big-number helpers (up to 4096 bit, 64 x u64 limbs, little-endian) ---------------
-constexpr int kHL = 64;
-struct UBig { uint64_t w[kHL]; };
+using namespace bftq::hostbig;
 
-bool ge(const UBig& a, const UBig& b) {
-  for (int i = kHL - 1; i >= 0; i--) { if (a.w[i] != b.w[i]) return a.w[i] > b.w[i]; }
-  return true;
-}
-void sub(UBig& a, const UBig& b) {
-  unsigned __int128 br = 0;
-  for (int i = 0; i < kHL; i++) {
-    unsigned __int128 d = (unsigned __int128)a.w[i] - b.w[i] - (uint64_t)br;
-    a.w[i] = (uint64_t)d;
-    br = (d >> 64) & 1;
-  }
-}
-// a = 2a mod n   (a < n on entry)
-void dbl_mod(UBig& a, const UBig& n) {
-  uint64_t top = a.w[kHL - 1] >> 63;
-  for (int i = kHL - 1; i > 0; i--) a.w[i] = (a.w[i] << 1) | (a.w[i - 1] >> 63);
-  a.w[0] <<= 1;
-  if (top || ge(a, n)) sub(a, n);
-}
-int bitlen(const UBig& a) {
-  for (int i = kHL - 1; i >= 0; i--) if (a.w[i]) return 64 * i + 64 - __builtin_clzll(a.w[i]);
-  return 0;
-}
-void from_be(UBig& a, const uint8_t* be, size_t len) {   // len bytes big-endian, len <= 512
-  memset(&a, 0, sizeof(a));
-  for (size_t i = 0; i < len; i++) {
-    const size_t bi = len - 1 - i;                        // little-endian byte number
-    a.w[bi >> 3] |= (uint64_t)be[i] << (8 * (bi & 7));
-  }
-}
 void to_digits(const UBig& a, uint32_t* d, int nd) {
   for (int i = 0; i < nd; i++) {
     int o = 28 * i;
@@ -774,18 +743,18 @@ int make_key_consts(const uint8_t* n_be, uint32_t stride, uint32_t exp, bftq::Rs
     while (exp2 < target) { dbl_mod(x, n); exp2++; }
     if (exp2 == target) to_digits(x, kd.r2[layout], bftq::kMaxDigits);
   }
-  // radix-2^32 constants (fast path, meaningful for exactly-2048-bit moduli): n, 2^4096 mod n, -n^-1 mod 2^32
+  // radix-2^32 constants (fast path, meaningful for exactly-2048-bit moduli): n, -n^-1 mod 2^32, the verification constants
   memset(&k32, 0, sizeof(k32));
-  for (int i = 0; i < 32; i++) { k32.n[2 * i] = (uint32_t)n.w[i]; k32.n[2 * i + 1] = (uint32_t)(n.w[i] >> 32); }
+  to_words(n, k32.n, 64);
   k32.n0inv = 0u - inv;
   k32.e = exp;
   k32.nbits = (uint32_t)nb;
   if (nb == 2048) {
-    UBig y;
-    memset(&y, 0, sizeof(y));
-    y.w[0] = 1;
-    for (int ex = 0; ex < 4096; ex++) dbl_mod(y, n);
-    for (int i = 0; i < 32; i++) { k32.r2[2 * i] = (uint32_t)y.w[i]; k32.r2[2 * i + 1] = (uint32_t)(y.w[i] >> 32); }
+    const bftq::hostbig::VerifyConsts vc = bftq::hostbig::verify_consts(n, exp);
+    to_words(vc.c16, k32.c16, 64);
+    to_words(vc.hc16, k32.hc16, 64);
+    to_words(vc.c32, k32.c32, 64);
+    to_words(vc.hc32, k32.hc32, 64);
   }
   if (is2048) *is2048 = !(cls == 256 && nb != 2048);
   return BFTQ_OK;

@@ -206,10 +206,12 @@ __device__ __forceinline__ void mont_finish(uint32_t (&out)[W], Acc<W>& A, const
 }
 
 // out = a * b * R^-1 mod n with R = 2^(128 W), out < R ("almost Montgomery").  a, b < R as W limbs/lane.
-// All 32 lanes of the warp must call this together.
+// owners < T stops after that many owner steps: out == a * b' * 2^(-32 W owners) (mod n) with b' the owners' low lanes of b, out < R
+// and, for a < n, out < 2n (K1's final check, one or two owner steps).  All 32 lanes of the warp must call this together.
 template <int W, bool STEP_SYNC = false, bool CT = false>
 __device__ __forceinline__ void mont_mul(uint32_t (&out)[W], const uint32_t (&a)[W], const uint32_t (&b)[W],
-                                         const uint32_t (&n)[W], const uint32_t n0inv, const int r, const int gbase) {
+                                         const uint32_t (&n)[W], const uint32_t n0inv, const int r, const int gbase,
+                                         const int owners = T) {
   Acc<W> A;
 #pragma unroll
   for (int k = 0; k < W + 4; k++) A.E[k] = 0u;
@@ -223,6 +225,7 @@ __device__ __forceinline__ void mont_mul(uint32_t (&out)[W], const uint32_t (&a)
   constexpr int kMulUnroll = BFTQ_MUL_UNROLL;      // owner steps per loop body (code size x this)
 #pragma unroll kMulUnroll
   for (int owner = 0; owner < T; owner++) {
+    if (owner == owners) break;                 // a full trip count keeps BFTQ_MUL_UNROLL free of remainder copies
     if (STEP_SYNC) __syncthreads();             // keep the block's warps in phase (see BFTQ_K1_SYNC)
     const int src = gbase + owner;
 #pragma unroll
@@ -282,12 +285,10 @@ __device__ __forceinline__ bool group_ge(const uint32_t (&x)[W], const uint32_t 
   return gtb >= ltb;
 }
 
-// x -= n when x >= n (x < 2n on entry).
+// d = x - y mod 2^(128 W) over the group's lanes; returns the borrow out of the top lane (the same in all four).
 template <int W>
-__device__ __forceinline__ void cond_sub(uint32_t (&x)[W], const uint32_t (&n)[W], const int r, const int gbase) {
-  const bool ge = group_ge(x, n, gbase);
-  uint32_t d[W];
-  const uint32_t bo = sub_n(d, x, n);
+__device__ __forceinline__ uint32_t group_sub(uint32_t (&d)[W], const uint32_t (&x)[W], const uint32_t (&y)[W], const int r, const int gbase) {
+  const uint32_t bo = sub_n(d, x, y);
   bool zeros = true;
 #pragma unroll
   for (int k = 0; k < W; k++) zeros = zeros && (d[k] == 0u);
@@ -296,6 +297,15 @@ __device__ __forceinline__ void cond_sub(uint32_t (&x)[W], const uint32_t (&n)[W
   uint32_t btop;
   const uint32_t bi = lane_carry_in(bgb, bpb, r, btop);
   ripple_sub(d, bi);
+  return btop;
+}
+
+// x -= n when x >= n (x < 2n on entry).
+template <int W>
+__device__ __forceinline__ void cond_sub(uint32_t (&x)[W], const uint32_t (&n)[W], const int r, const int gbase) {
+  const bool ge = group_ge(x, n, gbase);
+  uint32_t d[W];
+  group_sub(d, x, n, r, gbase);
   if (ge) {
 #pragma unroll
     for (int k = 0; k < W; k++) x[k] = d[k];
@@ -308,9 +318,12 @@ __device__ __forceinline__ void cond_sub(uint32_t (&x)[W], const uint32_t (&n)[W
 namespace bftq {
 namespace r32 {
 
-struct RsaKey32 {               // per key, radix 2^32 little-endian words
+struct RsaKey32 {               // per key, radix 2^32 little-endian words; c = R^-(e-1) mod n, R = 2^2048 (bignum_host.hpp)
   uint32_t n[64];
-  uint32_t r2[64];              // 2^4096 mod n
+  uint32_t c16[64];             // c * 2^512 mod n
+  uint32_t hc16[64];            // (EM with its low 512 bits cleared) * c mod n, for T of up to 63 bytes
+  uint32_t c32[64];             // c * 2^1024 mod n
+  uint32_t hc32[64];            // (EM with its low 1024 bits cleared) * c mod n, for longer T (SHA-384, SHA-512)
   uint32_t n0inv;               // -n^-1 mod 2^32
   uint32_t e;
   uint32_t nbits;
@@ -324,13 +337,20 @@ struct RsaKey32 {               // per key, radix 2^32 little-endian words
 #ifndef BFTQ_K1_SYNC
 #define BFTQ_K1_SYNC 2
 #endif
-// 1 = the exponentiation runs as one loop over a four-op program (one squaring and one product instance in the kernel
-// instead of the straight-line form's two squaring and three product instances), which keeps the hot loop small enough
+// 1 = the exponentiation runs as one loop over a three-op program (one squaring and one product instance in the kernel
+// instead of the straight-line form's one squaring and two product instances), which keeps the hot loop small enough
 // for the instruction caches (1 % faster than the straight-line form on H100, DESIGN.md §4).
 #ifndef BFTQ_K1_UNIFIED
 #define BFTQ_K1_UNIFIED 1
 #endif
 // SQ: the squarings of the exponentiation go through mont_sqr (rsa_square_r32.cuh) instead of mont_mul(y, y).
+//
+// The exponentiation never converts s to Montgomery form: it runs the square-and-multiply chain of e on the plain s,
+// every 1 bit below the top one a product with the plain s.  A squaring takes y = s^k R^-(k-1) to s^2k R^-(2k-1) and a
+// product with s to s^(k+1) R^-k, so the chain ends at Y = s^e c with c = R^-(e-1) mod n: 16 squarings and one product
+// for e = 65537.  With EM = H 2^k + L (k = 512, or 1024 for T longer than 63 bytes), s^e == EM (mod n) iff
+// Y == c L + hc (mod n); c L is ONE (or two) owner steps of mont_mul with the key's c * 2^k, and hc = H 2^k c mod n is
+// a per-key constant because H = 00 01 FF..FF does not depend on the digest (RsaKey32, bignum_host.hpp).
 template <int BLOCK, int MIN_BLOCKS, bool SQ>
 __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS)
 rsa_verify_r32_kernel(const RsaKey32* __restrict__ keys, const uint32_t nkeys, const uint32_t* __restrict__ key_idx,
@@ -339,9 +359,7 @@ rsa_verify_r32_kernel(const RsaKey32* __restrict__ keys, const uint32_t nkeys, c
                       uint8_t* __restrict__ status) {
   constexpr int W = 16;
   constexpr int kGroupsPerWarp = 32 / T;
-  // s*R mod n is only needed again for exponents with interior 1 bits (never for 65537): park it in
-  // shared memory instead of 16 registers.
-  __shared__ uint32_t xm_s[W][BLOCK];
+  __shared__ uint32_t y_s[W][BLOCK];
   __shared__ int nbmax_s;
   constexpr bool kStepSync = BFTQ_K1_SYNC >= 3;
   const int lane = threadIdx.x & 31;
@@ -349,6 +367,8 @@ rsa_verify_r32_kernel(const RsaKey32* __restrict__ keys, const uint32_t nkeys, c
   const int gbase = lane & ~(T - 1);
   const int plen = c_hash_prefix[hash_alg].len;
   const int dlen = c_hash_prefix[hash_alg].dlen;
+  const bool wide = plen + dlen > 63;                        // T and its 00 separator reach above 2^512: split EM at 2^1024
+  const int check_owners = wide ? 2 : 1;
   const uint64_t warp_global = (uint64_t)blockIdx.x * (BLOCK / 32) + (threadIdx.x >> 5);
   const uint64_t warps_total = (uint64_t)gridDim.x * (BLOCK / 32);
   const uint32_t gmask = ((1u << T) - 1u) << gbase;
@@ -373,6 +393,8 @@ rsa_verify_r32_kernel(const RsaKey32* __restrict__ keys, const uint32_t nkeys, c
     const uint32_t n0inv = __ldg(&key->n0inv);
     const uint32_t e = __ldg(&key->e);
     const uint8_t* sp = sig + item * (uint64_t)kRsaBytes;
+    const uint8_t* dp = digest + item * (uint64_t)dlen;
+    const uint32_t* ck = wide ? key->c32 : key->c16;
     bool s_ge_n;
 #pragma unroll
     for (int j = 0; j < W; j++) y[j] = be_word(sp, r * W + j);
@@ -389,12 +411,11 @@ rsa_verify_r32_kernel(const RsaKey32* __restrict__ keys, const uint32_t nkeys, c
       nbmax = nbmax_s;
     }
 #if BFTQ_K1_UNIFIED
-    // The whole exponentiation as ONE loop over a small program, so that the kernel holds a single instance of the
-    // squaring and a single instance of the general product (the straight-line form below has two and three: 75 KB of
-    // hot code per task instead of 31 KB; the instruction caches hold 32 KB).
-    //   op 0: y = s * R^2 (to Montgomery form; also parked as xm)      op 1: the squaring of `bit`
-    //   op 2: y *= xm after the squaring of an interior 1 bit            op 3: the last product, by the PLAIN s (or 1)
-    int op = 0, bit = nbmax - 2;
+    // The whole verification as ONE loop over a small program, so that the kernel holds a single instance of the
+    // squaring and a single instance of the general product (the straight-line form below has two products; the
+    // instruction caches hold 32 KB).
+    //   op 1: the squaring of `bit`      op 2: y *= s after the squaring of a 1 bit      op 3: the check product c L
+    int bit = nbmax - 2, op = bit >= 0 ? 1 : 3;
 #pragma unroll 1
     for (;;) {
       if (op == 1) {
@@ -404,50 +425,37 @@ rsa_verify_r32_kernel(const RsaKey32* __restrict__ keys, const uint32_t nkeys, c
 #pragma unroll
           for (int j = 0; j < W; j++) y[j] = t[j];
         }
-        const bool mul = bit >= 1 && bit <= nb - 2 && ((e >> bit) & 1u);
+        const bool mul = bit <= nb - 2 && ((e >> bit) & 1u);
         if (__any_sync(kFull, mul)) op = 2;
         else { bit--; op = bit >= 0 ? 1 : 3; }
       } else {
         uint32_t bop[W];
-        if (op == 0) {
+        if (op == 3) {
+          // b = EM's words (L in the owner lanes), built by a rolled loop through shared memory: one em_word instance
+          // instead of sixteen (2.7 K instructions).  Then Y waits in shared memory while y holds c * 2^k.
+#pragma unroll 1
+          for (int j = 0; j < W; j++) y_s[j][threadIdx.x] = em_word(r * W + j, dp, plen, dlen, hash_alg);
 #pragma unroll
-          for (int j = 0; j < W; j++) bop[j] = __ldg(&key->r2[r * W + j]);
-        } else if (op == 2) {
-#pragma unroll
-          for (int j = 0; j < W; j++) bop[j] = xm_s[j][threadIdx.x];
-        } else {                                              // plain s (bit 0 set) or plain 1: leaves Montgomery form
-#pragma unroll
-          for (int j = 0; j < W; j++) bop[j] = ((e & 1u) && nb >= 2) ? be_word(sp, r * W + j) : ((r == 0 && j == 0) ? 1u : 0u);
-        }
-        mont_mul(t, y, bop, nd, n0inv, r, gbase);
-        if (op == 3) break;
-        if (op == 0) {
-#pragma unroll
-          for (int j = 0; j < W; j++) { y[j] = t[j]; xm_s[j][threadIdx.x] = t[j]; }
-          op = bit >= 0 ? 1 : 3;
+          for (int j = 0; j < W; j++) { bop[j] = y_s[j][threadIdx.x]; y_s[j][threadIdx.x] = y[j]; y[j] = __ldg(&ck[r * W + j]); }
         } else {
-          if (bit <= nb - 2 && ((e >> bit) & 1u)) {
 #pragma unroll
-            for (int j = 0; j < W; j++) y[j] = t[j];
-          }
-          bit--;
-          op = bit >= 0 ? 1 : 3;
+          for (int j = 0; j < W; j++) bop[j] = be_word(sp, r * W + j);       // the plain s
         }
+        mont_mul(t, y, bop, nd, n0inv, r, gbase, op == 2 ? T : check_owners);
+        if (op == 3) break;
+        if (bit <= nb - 2 && ((e >> bit) & 1u)) {
+#pragma unroll
+          for (int j = 0; j < W; j++) y[j] = t[j];
+        }
+        bit--;
+        op = bit >= 0 ? 1 : 3;
       }
     }
+#pragma unroll
+    for (int j = 0; j < W; j++) y[j] = y_s[j][threadIdx.x];
 #else
-    {
-      uint32_t r2[W];
-#pragma unroll
-      for (int j = 0; j < W; j++) r2[j] = __ldg(&key->r2[r * W + j]);
-      mont_mul(t, y, r2, nd, n0inv, r, gbase);              // s * R mod n (almost reduced)
-#pragma unroll
-      for (int j = 0; j < W; j++) y[j] = t[j];
-    }
-#pragma unroll
-    for (int j = 0; j < W; j++) xm_s[j][threadIdx.x] = y[j];
 #pragma unroll 1
-    for (int bit = nbmax - 2; bit >= 1; bit--) {
+    for (int bit = nbmax - 2; bit >= 0; bit--) {
       const bool active = bit <= nb - 2;
       if (SQ) mont_sqr<kStepSync>(t, y, nd, n0inv, r, gbase); else mont_mul<W, kStepSync>(t, y, y, nd, n0inv, r, gbase);
       if (BFTQ_K1_SYNC >= 2) __syncthreads();
@@ -457,36 +465,37 @@ rsa_verify_r32_kernel(const RsaKey32* __restrict__ keys, const uint32_t nkeys, c
       }
       const bool mul = active && ((e >> bit) & 1u);
       if (__any_sync(kFull, mul)) {
-        uint32_t xm[W];
+        uint32_t sx[W];
 #pragma unroll
-        for (int j = 0; j < W; j++) xm[j] = xm_s[j][threadIdx.x];
-        mont_mul(t, y, xm, nd, n0inv, r, gbase);
+        for (int j = 0; j < W; j++) sx[j] = be_word(sp, r * W + j);
+        mont_mul(t, y, sx, nd, n0inv, r, gbase);
         if (mul) {
 #pragma unroll
           for (int j = 0; j < W; j++) y[j] = t[j];
         }
       }
     }
-    if (__any_sync(kFull, nb >= 2)) {
-      if (SQ) mont_sqr(t, y, nd, n0inv, r, gbase); else mont_mul(t, y, y, nd, n0inv, r, gbase);
-      if (nb >= 2) {
-#pragma unroll
-        for (int j = 0; j < W; j++) y[j] = t[j];
-      }
-    }
     {
-      uint32_t m1[W];                                       // plain s (bit 0 set) or plain 1
+      uint32_t ca[W], lb[W];
 #pragma unroll
-      for (int j = 0; j < W; j++) m1[j] = ((e & 1u) && nb >= 2) ? be_word(sp, r * W + j) : ((r == 0 && j == 0) ? 1u : 0u);
-      mont_mul(t, y, m1, nd, n0inv, r, gbase);            // plain operand: leaves Montgomery form
+      for (int j = 0; j < W; j++) { ca[j] = __ldg(&ck[r * W + j]); lb[j] = em_word(r * W + j, dp, plen, dlen, hash_alg); }
+      mont_mul(t, ca, lb, nd, n0inv, r, gbase, check_owners);
     }
 #endif
-    cond_sub(t, nd, r, gbase);                            // t < 2^2048 < 2n  ->  t mod n
-
-    const uint8_t* dp = digest + item * (uint64_t)dlen;
+    // y = Y < 2^2048 < 2n and t = Q == c L (mod n), Q < 2n.  With D = (Y mod n) - (Q mod n) mod 2^2048, borrow b, and
+    // F = hc - D mod 2^2048:  Y == Q + hc (mod n)  iff  F == 0 (b = 0: D = Y - Q in [0, n))  or  F == n (b = 1: D + n - 2^2048
+    // = Y - Q + n in (0, n)).
+    cond_sub(y, nd, r, gbase);
+    cond_sub(t, nd, r, gbase);
+    uint32_t d[W];
+    const uint32_t b = group_sub(d, y, t, r, gbase);
+    const uint32_t* hk = wide ? key->hc32 : key->hc16;
+#pragma unroll
+    for (int j = 0; j < W; j++) y[j] = __ldg(&hk[r * W + j]);
+    group_sub(t, y, d, r, gbase);
     bool eq = true;
 #pragma unroll
-    for (int j = 0; j < W; j++) eq = eq && (em_word(r * W + j, dp, plen, dlen, hash_alg) == t[j]);
+    for (int j = 0; j < W; j++) eq = eq && (t[j] == (b ? nd[j] : 0u));
     const uint32_t eqb = __ballot_sync(kFull, eq) & gmask;
     if (valid && r == 0) {
       uint8_t st = (eqb == gmask) ? (uint8_t)0 : (uint8_t)1;

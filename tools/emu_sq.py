@@ -51,7 +51,8 @@ def row_operand(a2, X, Y, j):
     return m, a_j
 
 
-def montsqr_emu(a, n, n0inv):
+def montsqr_acc(a, n, n0inv):
+    """the accumulators (E, O, Z, cin) after the four owner steps, and the a x a limb products per lane"""
     al = [[(a >> (32 * (r * W + j))) & M32 for j in range(W)] for r in range(T)]
     nl = [[(n >> (32 * (r * W + j))) & M32 for j in range(W)] for r in range(T)]
     a2 = []
@@ -97,6 +98,11 @@ def montsqr_emu(a, n, n0inv):
                 v = E[r][14] + (E[r][15] << 32) + (E[r][16] << 64) + (E[r][17] << 96) + r0 + (r1 << 32)
                 E[r][14] = v & M32; E[r][15] = (v >> 32) & M32; E[r][16] = (v >> 64) & M32; E[r][17] = (v >> 96) & M32
                 assert v >> 128 == 0
+    return E, O, Z, cin, nprod
+
+
+def montsqr_emu(a, n, n0inv):
+    E, O, Z, cin, nprod = montsqr_acc(a, n, n0inv)
     tot = 0
     for r in range(T):
         loc = cin[r] + Z[r] + sum(E[r][k] << (32 * k) for k in range(20)) + sum(O[r][k] << (32 * (k + 1)) for k in range(18))
