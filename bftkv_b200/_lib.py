@@ -88,6 +88,8 @@ def load():
         "bftq_message_decrypt_batch": (C.c_int, [vp, vp, vp, C.c_uint64, vp, vp, vp, vp, vp, vp, vp]),
         "bftq_keyring_add_private": (C.c_int, [vp, vp, C.c_uint64, u32p]),
         "bftq_read_responses_batch": (C.c_int, [vp, vp, C.c_uint32, vp, C.c_uint32, vp, C.c_uint64, vp, vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp, vp, vp, vp]),
+        "bftq_read_encrypted_responses_batch": (C.c_int, [vp, vp, C.c_uint32, vp, C.c_uint32, vp, C.c_uint64, vp, vp, vp, vp, vp, C.c_uint32, vp, vp, vp, vp,
+                                                          vp, vp, vp, vp, vp]),
         "bftq_signature_signers": (C.c_int, [vp, vp, C.c_uint64, vp, C.c_uint32, u32p]),
         "bftq_aggregator_create": (C.c_int, [vp, C.c_uint32, C.c_uint32, C.POINTER(vp)]),
         "bftq_aggregator_destroy": (None, [vp]),

@@ -359,11 +359,7 @@ class Message:
         return out
 
 
-def read_responses_batch(kr: "Keyring", qcs, op_off, peer_ids, msgs: Sequence[bytes], nonces, pre_status=None, blobs=None):
-    """Client.Read from raw answers (bftq_read_responses_batch).  qcs: [(f, min, threshold, suff, [node ids])]; op_off (n_ops+1)
-    uint32; peer_ids (N) uint64; msgs: N decrypted answers; nonces (N, nonce_len) uint8 — the nonces the requests carried.
-    blobs: (msg_blob, msg_off) arrays to use instead of joining `msgs` (e.g. page-locked ones).
-    Returns dict(status, ts, value_off, value_len, decision, winner, decided_at)."""
+def _read_args(qcs, op_off, peer_ids, msgs, nonces, pre_status, blobs):
     op_off = np.ascontiguousarray(op_off, np.uint32)
     n_ops, n = len(op_off) - 1, int(op_off[-1])
     arr = (QCIds * max(1, len(qcs)))()
@@ -374,16 +370,44 @@ def read_responses_batch(kr: "Keyring", qcs, op_off, peer_ids, msgs: Sequence[by
         off += len(m)
     mem = np.asarray(members if members else [0], np.uint64)
     blob, moff = blobs if blobs is not None else _blob(msgs)
-    peer_ids = np.ascontiguousarray(peer_ids, np.uint64)
     nonces = np.ascontiguousarray(nonces, np.uint8)
-    nonce_len = int(nonces.shape[1])
     pre = None if pre_status is None else np.ascontiguousarray(pre_status, np.uint8)
     out = {"status": np.zeros(max(n, 1), np.uint8), "ts": np.zeros(max(n, 1), np.uint64), "value_off": np.zeros(max(n, 1), np.uint32),
            "value_len": np.zeros(max(n, 1), np.uint32), "decision": np.zeros(n_ops, np.uint8), "winner": np.zeros(n_ops, np.uint32),
            "decided_at": np.zeros(n_ops, np.uint32)}
+    return op_off, n_ops, n, arr, mem, len(members), blob, moff, np.ascontiguousarray(peer_ids, np.uint64), nonces, pre, out
+
+
+def read_encrypted_responses_batch(kr: "Keyring", qcs, op_off, peer_ids, raws: Sequence[bytes], nonces, pre_status=None, blobs=None, want_plain=True):
+    """Client.Read from the raw wire answers (bftq_read_encrypted_responses_batch): as read_responses_batch, but each answer
+    is the encrypted transport message (PKESK + SEIPD) and the client's private key must be registered
+    (Keyring.register_private).  With want_plain the result also holds "plain": the good answers' plain texts (bytes, b""
+    for the others)."""
+    op_off, n_ops, n, arr, mem, n_mem, blob, moff, peer_ids, nonces, pre, out = _read_args(qcs, op_off, peer_ids, raws, nonces, pre_status, blobs)
+    pblob = np.zeros(max(int(moff[-1]) if len(moff) else 0, 1), np.uint8) if want_plain else None
+    plen = np.zeros(max(n, 1), np.uint32) if want_plain else None
     p = lambda a: C.c_void_p(a.ctypes.data) if a is not None else C.c_void_p(0)
-    _lib.check(kr._lib.bftq_read_responses_batch(kr._h, C.cast(arr, C.c_void_p), len(qcs), p(mem), len(members), p(op_off), n_ops, p(peer_ids), p(blob), p(moff),
-                                                 p(pre), p(nonces), nonce_len, p(out["status"]), p(out["ts"]), p(out["value_off"]), p(out["value_len"]),
+    _lib.check(kr._lib.bftq_read_encrypted_responses_batch(kr._h, C.cast(arr, C.c_void_p), len(qcs), p(mem), n_mem, p(op_off), n_ops, p(peer_ids), p(blob),
+                                                           p(moff), p(pre), p(nonces), int(nonces.shape[1]), p(out["status"]), p(out["ts"]),
+                                                           p(out["value_off"]), p(out["value_len"]), p(pblob), p(plen), p(out["decision"]),
+                                                           p(out["winner"]), p(out["decided_at"])))
+    for k in ("status", "ts", "value_off", "value_len"):
+        out[k] = out[k][:n]
+    if want_plain:
+        out["plain_len"] = plen[:n]
+        out["plain"] = [bytes(pblob[int(moff[i]):int(moff[i]) + int(plen[i])]) for i in range(n)]
+    return out
+
+
+def read_responses_batch(kr: "Keyring", qcs, op_off, peer_ids, msgs: Sequence[bytes], nonces, pre_status=None, blobs=None):
+    """Client.Read from raw answers (bftq_read_responses_batch).  qcs: [(f, min, threshold, suff, [node ids])]; op_off (n_ops+1)
+    uint32; peer_ids (N) uint64; msgs: N decrypted answers; nonces (N, nonce_len) uint8 — the nonces the requests carried.
+    blobs: (msg_blob, msg_off) arrays to use instead of joining `msgs` (e.g. page-locked ones).
+    Returns dict(status, ts, value_off, value_len, decision, winner, decided_at)."""
+    op_off, n_ops, n, arr, mem, n_mem, blob, moff, peer_ids, nonces, pre, out = _read_args(qcs, op_off, peer_ids, msgs, nonces, pre_status, blobs)
+    p = lambda a: C.c_void_p(a.ctypes.data) if a is not None else C.c_void_p(0)
+    _lib.check(kr._lib.bftq_read_responses_batch(kr._h, C.cast(arr, C.c_void_p), len(qcs), p(mem), n_mem, p(op_off), n_ops, p(peer_ids), p(blob), p(moff),
+                                                 p(pre), p(nonces), int(nonces.shape[1]), p(out["status"]), p(out["ts"]), p(out["value_off"]), p(out["value_len"]),
                                                  p(out["decision"]), p(out["winner"]), p(out["decided_at"])))
     for k in ("status", "ts", "value_off", "value_len"):
         out[k] = out[k][:n]

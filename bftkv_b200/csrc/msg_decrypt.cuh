@@ -388,7 +388,8 @@ __device__ bool decrypt_stream(const uint8_t* __restrict__ key, const uint8_t* _
 
 __device__ void seipd_item(const uint8_t* __restrict__ ct_blob, const uint64_t* __restrict__ ct_off, const uint32_t* __restrict__ cand_off,
                            const uint32_t* __restrict__ cand_rec, const uint8_t* __restrict__ rec_cipher, const uint8_t* __restrict__ keys,
-                           const uint64_t i, uint8_t* __restrict__ pt_blob, uint8_t* __restrict__ out_res, uint32_t* rk, uint32_t* wsh, const uint8_t* sb);
+                           const uint64_t i, uint8_t* __restrict__ pt_blob, uint8_t* __restrict__ out_res, const uint64_t* __restrict__ ct_end,
+                           uint32_t* rk, uint32_t* wsh, const uint8_t* sb);
 
 __device__ __forceinline__ int nk_of(uint8_t cipher) { return cipher == 7 ? 4 : (cipher == 8 ? 6 : 8); }
 
@@ -396,17 +397,21 @@ __device__ __forceinline__ int nk_of(uint8_t cipher) { return cipher == 7 ? 4 : 
 // candidate session keys are K6a records cand_rec[cand_off[i] .. cand_off[i+1]) with AES cipher ids rec_cipher[].
 // out_res[i]: 0 MDC good, 1 MDC bad, 2 no candidate passed the quick check, 3 a candidate passed but the packet is
 // too short to hold the MDC packet.  pt (same offsets as ct): the decrypted prefix | data | MDC packet.
+// ct_end (nullable): item i spans [ct_off[i], ct_end[i]) instead of [ct_off[i], ct_off[i+1]) — the items need not be
+// packed.  cand_off == nullptr: item i's one candidate is record i when rec_cipher[i] != 0, none otherwise (cand_rec
+// unused).
 __global__ void __launch_bounds__(K6B_BLOCK)
 seipd_decrypt_kernel(const uint8_t* __restrict__ ct_blob, const uint64_t* __restrict__ ct_off, const uint32_t* __restrict__ cand_off,
                      const uint32_t* __restrict__ cand_rec, const uint8_t* __restrict__ rec_cipher, const uint8_t* __restrict__ keys,
-                     const uint64_t n_items, uint8_t* __restrict__ pt_blob, uint8_t* __restrict__ out_res) {
+                     const uint64_t n_items, uint8_t* __restrict__ pt_blob, uint8_t* __restrict__ out_res,
+                     const uint64_t* __restrict__ ct_end = nullptr) {
   __shared__ uint8_t sb[256];
   __shared__ uint32_t rk[60 * K6B_BLOCK];
   __shared__ uint32_t wsh[K6B_BLOCK][17];         // SHA-1 schedule per thread, padded against bank conflicts
   for (int i = threadIdx.x; i < 256; i += blockDim.x) sb[i] = c_aes_sbox[i];
   __syncthreads();
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n_items) seipd_item(ct_blob, ct_off, cand_off, cand_rec, rec_cipher, keys, i, pt_blob, out_res, rk, wsh[threadIdx.x], sb);
+  if (i < n_items) seipd_item(ct_blob, ct_off, cand_off, cand_rec, rec_cipher, keys, i, pt_blob, out_res, ct_end, rk, wsh[threadIdx.x], sb);
 #pragma unroll 1
   for (int k = 0; k < 60; k++) rk[k * K6B_BLOCK + threadIdx.x] = 0u;    // no key schedule or plaintext left in shared memory
 #pragma unroll 1
@@ -414,12 +419,15 @@ seipd_decrypt_kernel(const uint8_t* __restrict__ ct_blob, const uint64_t* __rest
 }
 __device__ void seipd_item(const uint8_t* __restrict__ ct_blob, const uint64_t* __restrict__ ct_off, const uint32_t* __restrict__ cand_off,
                            const uint32_t* __restrict__ cand_rec, const uint8_t* __restrict__ rec_cipher, const uint8_t* __restrict__ keys,
-                           const uint64_t i, uint8_t* __restrict__ pt_blob, uint8_t* __restrict__ out_res, uint32_t* rk, uint32_t* wsh, const uint8_t* sb) {
+                           const uint64_t i, uint8_t* __restrict__ pt_blob, uint8_t* __restrict__ out_res, const uint64_t* __restrict__ ct_end,
+                           uint32_t* rk, uint32_t* wsh, const uint8_t* sb) {
   const uint8_t* ct = ct_blob + ct_off[i];
-  const uint64_t len = ct_off[i + 1] - ct_off[i];
+  const uint64_t len = (ct_end != nullptr ? ct_end[i] : ct_off[i + 1]) - ct_off[i];
   int chosen = -1;
-  for (uint32_t c = cand_off[i]; c < cand_off[i + 1] && chosen < 0; c++) {
-    const uint32_t rec = cand_rec[c];
+  const uint32_t c0 = cand_off != nullptr ? cand_off[i] : (uint32_t)i;
+  const uint32_t c1 = cand_off != nullptr ? cand_off[i + 1] : (uint32_t)i + (rec_cipher[i] != 0 ? 1u : 0u);
+  for (uint32_t c = c0; c < c1 && chosen < 0; c++) {
+    const uint32_t rec = cand_off != nullptr ? cand_rec[c] : c;
     const uint8_t* key = keys + (uint64_t)rec * 32u;
     const int nk = nk_of(rec_cipher[rec]);
     const bool pass = nk == 4 ? quick_check<4>(key, ct, rk, sb) : (nk == 6 ? quick_check<6>(key, ct, rk, sb) : quick_check<8>(key, ct, rk, sb));
@@ -432,6 +440,139 @@ __device__ void seipd_item(const uint8_t* __restrict__ ct_blob, const uint64_t* 
   const int nk = nk_of(rec_cipher[chosen]);
   const bool ok = nk == 4 ? decrypt_stream<4>(key, ct, len, pt, rk, wsh, sb) : (nk == 6 ? decrypt_stream<6>(key, ct, len, pt, rk, wsh, sb) : decrypt_stream<8>(key, ct, len, pt, rk, wsh, sb));
   out_res[i] = ok ? 0 : 1;
+}
+
+
+// ---- K6p / K6q: the decryption front stage of the encrypted read path (bftq_read_encrypted_responses_batch) ----------
+// K6p decides, per raw answer, whether it has the shape every bftkv answer has on the wire (Message.Encrypt,
+// crypto_pgp.go:418-437): exactly one PKESK (new-format header, definite length, v3, RSA, a non-wildcard key id whose
+// decryption the host's key loop would hand to exactly one registered private key, an MPI of at most 256 bytes ending the
+// packet) followed by one SEIPD v1 (new-format header, definite or partial lengths, ending exactly at the end of the
+// message, at least 40 body bytes after the version byte).  Such an answer gets c and its key slot for K6a and its
+// de-chunked SEIPD body for K6b; c > n (rsa.decrypt's ErrDecryption) is decided here against the slot's public modulus.
+// Every other shape goes to the host path whole: the flag, not a guess, decides.
+struct KeySlot { uint64_t key_id; uint32_t slot; uint32_t pad; };
+constexpr uint8_t kFrontDevice = 0, kFrontHost = 1, kFrontDecided = 2;
+constexpr uint8_t kStDecryptFailed = 10, kStUnsupported = 5, kStHostPlaceholder = 6;
+
+// One thread per answer.  raw_off: absolute offsets, raw_base: the offset of raw[0].  Per answer i (o0 = raw_off[i] -
+// raw_base): out_state / out_pre (kFrontDecided: pre is the final status; kFrontHost: pre = a placeholder K0m skips),
+// out_slot + out_c (n x 256, c left-padded, zero unless on the device), the de-chunked body at ct_blob + o0 spanning
+// [out_ct_beg[i], out_ct_end[i]) (relative to ct_blob), out_inner_end[i] = the absolute end K0m sees when it reads the
+// decrypted stream from pt_blob + 18 with the same raw_off.  Stores no secret: it reads the slots' public moduli only.
+__global__ void __launch_bounds__(128)
+pkesk_seipd_parse_kernel(const uint8_t* __restrict__ raw, const uint64_t* __restrict__ raw_off, const uint64_t raw_base, const uint32_t n_items,
+                         const uint8_t* __restrict__ pre_in /* nullable */, const KeySlot* __restrict__ tab, const uint32_t n_tab,
+                         const RsaPriv32* __restrict__ keys, uint32_t* __restrict__ out_slot, uint8_t* __restrict__ out_c,
+                         uint8_t* __restrict__ ct_blob, uint64_t* __restrict__ out_ct_beg, uint64_t* __restrict__ out_ct_end,
+                         uint64_t* __restrict__ out_inner_end, uint8_t* __restrict__ out_state, uint8_t* __restrict__ out_pre,
+                         uint8_t* __restrict__ out_cipher) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_items) return;
+  const uint64_t o0 = raw_off[i] - raw_base, o1 = raw_off[i + 1] - raw_base;
+  const uint8_t* m = raw + o0;
+  const uint8_t given = pre_in != nullptr ? pre_in[i] : (uint8_t)0;
+  uint8_t state = kFrontHost, pre = kStHostPlaceholder;
+  uint32_t slot = n_tab ? tab[0].slot : 0u, mpi_at = 0, ml = 0;
+  uint64_t L = 0;
+  if (given != 0) { state = kFrontDecided; pre = given; }
+  else if (o1 - o0 >= 64 && o1 - o0 <= 0x3fffffffull && n_tab) {
+    const uint32_t n = (uint32_t)(o1 - o0);
+    bool ok = m[0] == 0xC1;
+    // ---- PKESK: definite new-format length
+    uint32_t p = 1, bl = 0;
+    if (ok) {
+      const uint8_t o = m[1];
+      if (o < 192) { bl = o; p = 2; }
+      else if (o < 224) { bl = ((uint32_t)(o - 192) << 8) + m[2] + 192; p = 3; }
+      else if (o == 255) { bl = ((uint32_t)m[2] << 24) | ((uint32_t)m[3] << 16) | ((uint32_t)m[4] << 8) | m[5]; p = 6; }
+      else ok = false;
+      ok = ok && bl <= n - p && bl >= 12;
+    }
+    uint64_t kid = 0;
+    if (ok) {
+      const uint8_t* b = m + p;
+      for (int k = 1; k < 9; k++) kid = (kid << 8) | b[k];
+      ml = ((((uint32_t)b[10] << 8) | b[11]) + 7) / 8;
+      ok = b[0] == 3 && kid != 0 && (b[9] == 1 || b[9] == 2) && ml <= 256 && 12 + ml == bl;
+      mpi_at = p + 12;
+    }
+    if (ok) {
+      int hit = -1;
+      for (uint32_t k = 0; k < n_tab; k++) if (tab[k].key_id == kid) { hit = (int)k; break; }
+      ok = hit >= 0;
+      if (ok) slot = tab[hit].slot;
+    }
+    // ---- SEIPD: the rest of the message, de-chunked behind the version byte
+    uint32_t q = p + bl;
+    ok = ok && q + 2 <= n && m[q] == 0xD2;
+    q++;
+    bool last = false, first = true;
+    uint8_t* ct = ct_blob + o0;
+    while (ok && !last) {
+      const uint8_t o = m[q];
+      uint32_t l;
+      if (o < 192) { l = o; q += 1; last = true; }
+      else if (o < 224) { if (q + 2 > n) { ok = false; break; } l = ((uint32_t)(o - 192) << 8) + m[q + 1] + 192; q += 2; last = true; }
+      else if (o == 255) { if (q + 5 > n) { ok = false; break; } l = ((uint32_t)m[q + 1] << 24) | ((uint32_t)m[q + 2] << 16) | ((uint32_t)m[q + 3] << 8) | m[q + 4]; q += 5; last = true; }
+      else { l = 1u << (o & 0x1f); q += 1; }
+      if (l > n - q || (!last && q + l >= n)) { ok = false; break; }
+      uint32_t k = 0;
+      if (first && l > 0) { ok = m[q] == 1; k = 1; first = false; }
+      for (; k < l; k++) ct[L++] = m[q + k];
+      q += l;
+    }
+    ok = ok && !first && q == n && L >= 40;
+    if (ok) {
+      // c left-padded into K6a's layout, then c > n against the slot's modulus (most significant word first)
+      uint8_t* c = out_c + (uint64_t)i * 256u;
+      for (uint32_t k = 0; k < 256u - ml; k++) c[k] = 0;
+      for (uint32_t k = 0; k < ml; k++) c[256u - ml + k] = m[mpi_at + k];
+      int cmp = 0;
+      for (uint32_t j = 0; j < 256u && cmp == 0; j++) {
+        const uint32_t cb = j < 256u - ml ? 0u : m[mpi_at + j - (256u - ml)];
+        const uint32_t nb = (__ldg(&keys[slot].n[63 - j / 4]) >> (8 * (3 - j % 4))) & 0xffu;
+        cmp = cb > nb ? 1 : (cb < nb ? -1 : 0);
+      }
+      if (cmp > 0) { state = kFrontDecided; pre = kStDecryptFailed; }
+      else { state = kFrontDevice; pre = 0; }
+    }
+  }
+  if (state != kFrontDevice) {
+    uint32_t* c = reinterpret_cast<uint32_t*>(out_c + (uint64_t)i * 256u);
+    for (int k = 0; k < 64; k++) c[k] = 0u;
+    L = 0;
+  }
+  out_slot[i] = slot;
+  out_ct_beg[i] = o0;
+  out_ct_end[i] = o0 + L;
+  out_inner_end[i] = state == kFrontDevice ? raw_off[i] + L - 40 : raw_off[i];
+  out_state[i] = state;
+  out_pre[i] = pre;
+  out_cipher[i] = 0;
+}
+
+// K6q, one thread per answer, between the front stage's kernels.  stage 0 (after K6a): EncryptedKey.Decrypt's outcome
+// and FindKey's checks as bftq_message_decrypt_batch applies them to one PKESK — no key (invalid padding, c > n) or a
+// message shorter than 3 bytes, an unknown cipher or a wrong key length: ErrDecryptionFailed; 3DES / CAST5: handed back
+// (UNSUPPORTED); otherwise the AES cipher id for K6b.  stage 1 (after K6b): the quick check failed -> ErrDecryptionFailed;
+// an MDC mismatch goes to the host, which knows whether ReadAll reaches the MDC.
+__global__ void __launch_bounds__(256)
+front_gate_kernel(const int stage, const uint32_t n_items, const uint32_t* __restrict__ info, const uint8_t* __restrict__ res,
+                  uint8_t* __restrict__ state, uint8_t* __restrict__ pre, uint8_t* __restrict__ cipher_out) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_items || state[i] != kFrontDevice) return;
+  if (stage == 0) {
+    const uint32_t w = info[i], st = w & 0xff, cipher = (w >> 8) & 0xff, klen = w >> 16;
+    const uint32_t ks = cipher == 2 || cipher == 8 ? 24u : (cipher == 3 || cipher == 7 ? 16u : (cipher == 9 ? 32u : 0u));
+    if (st != kDecOk || ks == 0 || ks != klen) { state[i] = kFrontDecided; pre[i] = kStDecryptFailed; }
+    else if (cipher == 2 || cipher == 3) { state[i] = kFrontDecided; pre[i] = kStUnsupported; }
+    else cipher_out[i] = (uint8_t)cipher;
+  } else {
+    const uint8_t r = res[i];
+    if (r == 1) { state[i] = kFrontHost; pre[i] = kStHostPlaceholder; }
+    else if (r != 0) { state[i] = kFrontDecided; pre[i] = kStDecryptFailed; }
+  }
 }
 
 }  // namespace k6

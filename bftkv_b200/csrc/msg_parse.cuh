@@ -73,7 +73,7 @@ msg_parse_digest_kernel(const uint8_t* __restrict__ msg_blob, const uint64_t* __
                         uint32_t* __restrict__ out_key_idx, uint8_t* __restrict__ out_sig /* n x 256 */, uint8_t* __restrict__ out_digest /* n x 32 */,
                         uint8_t* __restrict__ out_pre, uint8_t* __restrict__ out_where, uint8_t* __restrict__ out_aux, uint64_t* __restrict__ out_ts,
                         uint32_t* __restrict__ out_voff, uint32_t* __restrict__ out_vlen, uint32_t* __restrict__ out_plen,
-                        uint64_t* __restrict__ out_signed_by) {
+                        uint64_t* __restrict__ out_signed_by, const uint64_t* __restrict__ msg_end = nullptr /* item i ends at msg_end[i], not msg_off[i+1] */) {
   // the SHA-256 message block of every thread lives in shared memory (word-major: conflict-free), so the byte stream can be
   // absorbed with a dynamic word index without spilling sixteen registers to local memory
   __shared__ uint32_t w_s[16][128];
@@ -81,7 +81,7 @@ msg_parse_digest_kernel(const uint8_t* __restrict__ msg_blob, const uint64_t* __
   const bool live = item_raw < n_items;
   const uint32_t item = live ? item_raw : n_items - 1;
   const int lane = threadIdx.x & 31;
-  const uint64_t o0 = msg_off[item] - msg_base, o1 = msg_off[item + 1] - msg_base;
+  const uint64_t o0 = msg_off[item] - msg_base, o1 = (msg_end != nullptr ? msg_end[item] : msg_off[item + 1]) - msg_base;
   const uint8_t* m = msg_blob + o0;
   uint8_t* plain = plain_blob + ((o0 + 3) & ~(uint64_t)3);        // 4-byte aligned inside the item's span (the fast path stores words)
   uint8_t where = kParseDecided, pre = 0, aux = 0;
@@ -282,6 +282,22 @@ msg_parse_digest_kernel(const uint8_t* __restrict__ msg_blob, const uint64_t* __
     out_ts[item] = ts; out_voff[item] = voff; out_vlen[item] = vlen; out_plen[item] = plen;
     if (out_signed_by != nullptr) out_signed_by[item] = signed_by;
   }
+}
+
+// The plain text of every good answer (status OK / UNVERIFIED_SIGNER), one warp per answer: plain_len[i] bytes from
+// plain_ptr[i] to out + (off[i] - base), the rest of the answer's span zeroed; out_len[i] = that length (0 otherwise).
+__global__ void __launch_bounds__(256)
+plain_gather_kernel(const uint8_t* __restrict__ status, const uint64_t* __restrict__ plain_ptr, const uint32_t* __restrict__ plain_len,
+                    const uint64_t* __restrict__ off, const uint64_t base, const uint32_t n_items, uint8_t* __restrict__ out, uint32_t* __restrict__ out_len) {
+  const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (i >= n_items) return;
+  const uint64_t o0 = off[i] - base, span = off[i + 1] - off[i];
+  const uint8_t st = status[i];
+  const uint32_t len = (st == 0 || st == kStUnverifiedSigner) ? plain_len[i] : 0u;
+  const uint8_t* src = reinterpret_cast<const uint8_t*>(plain_ptr[i]);
+  for (uint64_t k = lane; k < span; k += 32) out[o0 + k] = k < len ? src[k] : (uint8_t)0;
+  if (lane == 0) out_len[i] = len;
 }
 
 // K2m: one warp per operation (<= 32 responders).  status[] holds K1's verdicts (or the host packer's for the flagged

@@ -400,3 +400,54 @@ def make_read_answers(n_ops: int, n_replicas: int, seed: int = 0xBF7C0007, ss_si
     return {"keyring": b"".join(blocks), "ids": kids, "op_off": op_off, "peer_ids": np.array(kids, np.uint64)[key_idx], "msgs": msgs,
             "nonces": nonces, "pre_status": pre, "expect_status": expect, "ts": ts, "value_id": np.where(kind == 1, 1, 0).astype(np.uint32),
             "key_idx": key_idx}
+
+
+# ---- the encryption layer: what Message.Encrypt (crypto_pgp.go:418-437) puts on the wire around an answer -------------
+def secret_key_packet(k, ctime: int = 0x5E000000) -> bytes:
+    """RFC 4880 §5.5.3 secret-key packet (tag 5), v4, RSA, S2K usage 0: what Keyring.register_private takes.  The key id
+    equals pgp_public_key_block's for the same key and ctime."""
+    pub = bytes([4]) + struct.pack(">I", ctime) + bytes([1]) + _mpi(k["n"]) + _mpi(k["e"])
+    sec = _mpi(k["d"]) + _mpi(k["p"]) + _mpi(k["q"]) + _mpi(pow(k["p"], -1, k["q"]))
+    return _new_packet(5, pub + bytes([0]) + sec + struct.pack(">H", sum(sec) & 0xFFFF))
+
+
+ENC_FLIP, ENC_BAD_QUICK = 1, 2        # encrypt_answers' fault kinds
+
+
+def encrypt_answers(msgs, client_key, client_id: int, seed: int = 0xBF7C0008, cipher: int = 7, p_flip: float = 0.0, p_bad_quick: float = 0.0):
+    """Each non-empty inner message (make_read_answers' msgs) as openpgp.Encrypt writes it to the client: one PKESK v3
+    (RSA, PKCS#1 v1.5 type 2 around cipher | session key | checksum) to client_id, then one SEIPD v1 in Go's partial
+    lengths over OpenPGP CFB (zero IV, no resync: plain CFB128) of prefix | inner | MDC packet.  cipher: 7 / 8 / 9 =
+    AES-128 / 192 / 256.  Faults: ENC_FLIP flips one ciphertext byte of the MDC (ReadAll's MDC error), ENC_BAD_QUICK breaks
+    the quick check.  Empty messages (no answer) stay empty.  Returns (raws, fault) with fault an (N,) uint8 array."""
+    from cryptography.hazmat.primitives.ciphers import Cipher, algorithms
+    try:
+        from cryptography.hazmat.decrepit.ciphers.modes import CFB
+    except ImportError:
+        from cryptography.hazmat.primitives.ciphers.modes import CFB
+    rng = np.random.default_rng(seed)
+    ks = {7: 16, 8: 24, 9: 32}[cipher]
+    n, e = client_key["n"], client_key["e"]
+    N = len(msgs)
+    u = rng.random(N)
+    fault = np.where(u < p_flip, ENC_FLIP, np.where(u < p_flip + p_bad_quick, ENC_BAD_QUICK, 0)).astype(np.uint8)
+    head = bytes([3]) + struct.pack(">Q", client_id) + bytes([1])
+    out = []
+    for i, inner in enumerate(msgs):
+        if not inner:
+            out.append(b"")
+            continue
+        key = rng.bytes(ks)
+        block = bytes([cipher]) + key + struct.pack(">H", sum(key) & 0xFFFF)
+        ps = bytes(rng.integers(1, 256, 256 - 3 - len(block), dtype=np.uint8))
+        c = pow(int.from_bytes(b"\x00\x02" + ps + b"\x00" + block, "big"), e, n)
+        prefix = rng.bytes(16)
+        prefix += prefix[14:16] if fault[i] != ENC_BAD_QUICK else bytes([prefix[14] ^ 1, prefix[15]])
+        body = prefix + inner + b"\xd3\x14"
+        body += hashlib.sha1(body).digest()
+        enc = Cipher(algorithms.AES(key), CFB(bytes(16))).encryptor()
+        ct = bytearray(enc.update(body) + enc.finalize())
+        if fault[i] == ENC_FLIP:
+            ct[len(ct) - 1 - int(rng.integers(0, 20))] ^= 0x01       # inside the MDC: the inner stream stays intact
+        out.append(_new_packet(1, head + _mpi(c)) + bytes([0xC0 | 18]) + go_partial_write(b"\x01" + bytes(ct)) + b"\x00")
+    return out, fault

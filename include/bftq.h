@@ -64,6 +64,8 @@ extern "C" {
 #define BFTQ_ST_NONCE_MISMATCH  7   /* transport.ErrTransportNonceMismatch (transport.go:121-124)  */
 #define BFTQ_ST_UNVERIFIED_SIGNER 8 /* ACCEPTED, as the reference accepts it: the message's signer is not in the keyring, so
                                        openpgp.ReadMessage leaves SignedBy nil and never checks the signature (read path only) */
+#define BFTQ_ST_DECRYPT_FAILED 10  /* Decrypt returned crypto.ErrDecryptionFailed (ReadMessage failed: no PKESK key decrypts,
+                                      quick check, SEIPD framing, inner-stream framing) or ReadAll's MDC error (encrypted read path only) */
 
 /* ---- hash algorithm ids = OpenPGP ids (RFC 4880 §9.4), as sig.Hash in x/crypto ---------------*/
 #define BFTQ_HASH_MD5        1
@@ -498,6 +500,29 @@ int bftq_read_responses_batch(bftq_keyring* kr, const bftq_qc_ids_t* qcs, uint32
                               const uint8_t* pre_status, const uint8_t* nonce_blob, uint32_t nonce_len, uint8_t* out_status, uint64_t* out_ts,
                               uint32_t* out_value_off, uint32_t* out_value_len, uint8_t* out_decision, uint32_t* out_winner, uint32_t* out_decided_at);
 
+/* The read path from the raw wire answers: bftq_read_responses_batch with PGPMessage.Decrypt's encryption layer in front.
+ * Arguments, limits and argument errors are those of bftq_read_responses_batch; response p is the raw answer as
+ * transport.Multicast receives it (PKESK(s) + SEIPD, what Message.Encrypt writes), at raw_blob + raw_off[p].  The client's
+ * private key must have been registered with bftq_keyring_add_private.  The status of an answer follows the code
+ * bftq_message_decrypt_batch returns for the same bytes: pre_status non-zero is kept; 0 -> OK / UNVERIFIED_SIGNER, then
+ * NONCE_MISMATCH, then MALFORMED when packet.Parse fails (as bftq_read_responses_batch); BFTQ_ERR_INVALID_SIGNATURE ->
+ * BAD_SIGNATURE or HASH_TAG; BFTQ_ERR_MALFORMED, BFTQ_ERR_MDC -> BFTQ_ST_DECRYPT_FAILED; BFTQ_ERR_NOT_SIGNED,
+ * BFTQ_ERR_MESSAGE_BODY -> MALFORMED (so a signed but unencrypted answer fails here); BFTQ_ERR_UNSUPPORTED -> UNSUPPORTED.
+ * On the device (K6p parse -> K6a RSA-CRT -> K6b AES-CFB / MDC -> K0m -> K1 -> K2m) for the shape every bftkv answer has:
+ * one PKESK v3 to a key with exactly one registered private half, one SEIPD v1 to the end of the message.  Every other
+ * answer, and every one whose MDC does not match, runs whole through bftq_message_decrypt_batch and is patched in.
+ *   out_plain_blob / out_plain_len (nullable pair)  each good answer's plain text (what Decrypt returns) at
+ *                     out_plain_blob + raw_off[p], out_plain_len[p] bytes (0 for the other answers, whose span is zeroed);
+ *                     out_value_off is relative to it.
+ * Decrypted plain text left in the library's device scratch is not scrubbed (as bftq_message_decrypt_batch); session keys
+ * live in a per-call allocation zeroed before the call returns. */
+int bftq_read_encrypted_responses_batch(bftq_keyring* kr, const bftq_qc_ids_t* qcs, uint32_t n_qc, const uint64_t* member_ids, uint32_t n_members,
+                                        const uint32_t* op_off, uint64_t n_ops, const uint64_t* peer_ids, const uint8_t* raw_blob, const uint64_t* raw_off,
+                                        const uint8_t* pre_status, const uint8_t* nonce_blob, uint32_t nonce_len,
+                                        uint8_t* out_status, uint64_t* out_ts, uint32_t* out_value_off, uint32_t* out_value_len,
+                                        uint8_t* out_plain_blob, uint32_t* out_plain_len,
+                                        uint8_t* out_decision, uint32_t* out_winner, uint32_t* out_decided_at);
+
 /* ---- quorum-descriptor builder (host only; no GPU needed) --------------------------------------
  * The step before the tally: wotqs.ChooseQuorum over the PGP trust graph
  * (quorum/wotqs/wotqs.go:36-127, node/graph/graph.go:46-75,117-125,279-393,420-438).  The shim
@@ -551,8 +576,9 @@ typedef struct {
   uint64_t packer_wait_ns;   /* waiting for a chunk's results                                          */
   int32_t  numa_node;        /* NUMA node of the engine's GPU (-1 unknown)                             */
   uint32_t numa_cpus;        /* CPUs the library's worker threads are bound to (0 = not bound)         */
-  uint64_t msg_gpu_items;    /* transport answers parsed + hashed on the GPU (K0m) by bftq_read_responses_batch   */
-  uint64_t msg_host_items;   /* ... and the ones K0m flagged, decided through the host packer                    */
+  uint64_t msg_gpu_items;    /* transport answers decided on the GPU by bftq_read_responses_batch (K0m) and
+                                bftq_read_encrypted_responses_batch (K6p .. K0m)                                  */
+  uint64_t msg_host_items;   /* ... and the ones those kernels flagged, decided through the host packer / decrypt path */
   uint64_t unsupported_items;/* tuples answered BFTQ_ST_NOT_BUILT by the packer: key sizes / curves the reference's
                                 library can verify and this build cannot (INTEGRATION.md "fallback")              */
 } bftq_stats_t;
