@@ -4,7 +4,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("BFTQ_LIB_PATH") or os.path.join(_HERE, "libbftq.so")     # BFTQ_LIB_PATH: kernel-variant experiments (tools/)
+LIB_PATH = os.environ.get("BFTQ_LIB_PATH") or os.path.join(_HERE, "libbftq.so")     # BFTQ_LIB_PATH: load another build, e.g. a parent commit's, for an A/B timing run
 
 
 class BftqError(RuntimeError):

@@ -180,7 +180,6 @@ struct bftq_engine {
   // Montgomery constants of keys that arrive with a call (VerifyWithCertificate's presented certificate): a bounded
   // host-side cache, never entered in the device table above (an unauthenticated presenter must not grow engine state)
   std::map<std::string, std::pair<bftq::RsaKeyDev, bftq::r32::RsaKey32>> cert_consts;
-  int rsa_kernel = 0;                            // 0 auto, 28 force radix-2^28, 32 radix-2^32 without / 33 with the dedicated squaring (env BFTQ_RSA_KERNEL)
   std::vector<StagingSlot*> slots;
   bftq_stats_t stats{};
   std::map<std::string, uint32_t> key_lookup;   // (modulus bytes || e) -> key table index
@@ -196,8 +195,6 @@ struct bftq_engine {
   cpu_set_t numa_cpus;
   std::map<void*, size_t> host_allocs;           // bftq_host_alloc blocks
   uint32_t packer_flags = 0;   // BFTQ_F_* the packet-level entry points pass to K1 (bftq_engine_set_verify_flags / env BFTQ_STRICT_RANGE)
-  int rsa_t = 4;          // lanes per signature (env BFTQ_RSA_T)
-  int rsa_block = 128;
   std::mutex kr_mu;
   std::vector<bftq_keyring*> keyrings;           // live keyrings: their private-key tables are zeroed at shutdown
 };
@@ -509,41 +506,26 @@ int launch_rsa_any(bftq_engine* e, const KeyView& kv, const uint32_t* d_key_idx,
     e->stats.items += n_items;
   }
   const bool fits32 = exact2048 < 0 ? kv.all_2048 : exact2048 == 1;
-  const bool use32 = kb == 256 && fits32 && e->rsa_kernel != 28;
-  if (kb == 256 && !fits32 && (e->rsa_kernel == 32 || e->rsa_kernel == 33)) return fail(BFTQ_ERR_UNSUPPORTED_KEY, "radix-2^32 kernel forced but a modulus of the batch is not 2048 bits");
-  if (use32) {
-    // rsa_kernel 32 = general products only (mont_mul(y, y)); default / 33 = the squarings go through mont_sqr
-    const bool sq = e->rsa_kernel != 32;
-    static const int min_blocks = [] { const char* v = getenv("BFTQ_R32_BLOCKS"); return v ? atoi(v) : 4; }();
-    using kern_t = void (*)(const bftq::r32::RsaKey32*, uint32_t, const uint32_t*, const uint8_t*, const uint8_t*, uint32_t, uint64_t, uint32_t,
-                            const uint8_t*, uint8_t*);
-#ifndef BFTQ_K1_BLOCK
-#define BFTQ_K1_BLOCK 128
-#endif
-    constexpr int kBlk = BFTQ_K1_BLOCK, kMinB = 512 / BFTQ_K1_BLOCK;      // 16 warps per SM either way
-    kern_t kern = sq ? (min_blocks == 3 ? (kern_t)bftq::r32::rsa_verify_r32_kernel<128, 3, true> : (kern_t)bftq::r32::rsa_verify_r32_kernel<kBlk, kMinB, true>)
-                     : (min_blocks == 3 ? (kern_t)bftq::r32::rsa_verify_r32_kernel<128, 3, false> : (kern_t)bftq::r32::rsa_verify_r32_kernel<kBlk, kMinB, false>);
-    const int blk = min_blocks == 3 ? 128 : kBlk;
+  if (kb == 256 && fits32) {
+    constexpr int blk = bftq::r32::kK1Block;
     static thread_local int occ32 = 0;
-    if (!occ32) { CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ32, kern, blk, 0)); if (occ32 < 1) occ32 = 1; }
+    if (!occ32) { CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ32, bftq::r32::rsa_verify_r32_kernel, blk, 0)); if (occ32 < 1) occ32 = 1; }
     const uint64_t per_block = (uint64_t)(blk / 32) * 8;
     uint64_t grid = std::min<uint64_t>((n_items + per_block - 1) / per_block, (uint64_t)e->sm_count * occ32);
     if (grid < 1) grid = 1;
-    kern<<<(unsigned)grid, blk, 0, st>>>(kv.d_keys32, kv.nkeys, d_key_idx, d_sig, d_digest, hash_alg, n_items, flags,
-                                         d_pre, d_status);
+    bftq::r32::rsa_verify_r32_kernel<<<(unsigned)grid, blk, 0, st>>>(kv.d_keys32, kv.nkeys, d_key_idx, d_sig, d_digest, hash_alg,
+                                                                      n_items, flags, d_pre, d_status);
     CU(cudaGetLastError());
     return BFTQ_OK;
   }
   switch (kb) {
     case 128: return launch_rsa<4, 10, 128, 128>(e, kv, d_key_idx, d_sig, d_digest, hash_alg, n_items, flags, d_pre, d_status, st);
     case 192: return launch_rsa<4, 14, 128, 192>(e, kv, d_key_idx, d_sig, d_digest, hash_alg, n_items, flags, d_pre, d_status, st);
+    case 256: return launch_rsa<4, 19, 128, 256>(e, kv, d_key_idx, d_sig, d_digest, hash_alg, n_items, flags, d_pre, d_status, st);
     case 384: return launch_rsa<8, 14, 128, 384>(e, kv, d_key_idx, d_sig, d_digest, hash_alg, n_items, flags, d_pre, d_status, st);
     case 512: return launch_rsa<8, 19, 128, 512>(e, kv, d_key_idx, d_sig, d_digest, hash_alg, n_items, flags, d_pre, d_status, st);
-    case 256: break;
     default: return fail(BFTQ_ERR_UNSUPPORTED_KEY, "key size class not built (128/192/256/384/512 bytes are)");
   }
-  if (e->rsa_t == 8) return launch_rsa<8, 10, 128, 256>(e, kv, d_key_idx, d_sig, d_digest, hash_alg, n_items, flags, d_pre, d_status, st);
-  return launch_rsa<4, 19, 128, 256>(e, kv, d_key_idx, d_sig, d_digest, hash_alg, n_items, flags, d_pre, d_status, st);
 }
 
 // ---- integer-pipe peak micro-benchmark ---------------------------------------------------------
@@ -617,15 +599,6 @@ int bftq_init(int device, bftq_engine** out) {
   auto* e = new bftq_engine();
   e->device = device;
   e->sm_count = prop.multiProcessorCount;
-  if (const char* k = getenv("BFTQ_RSA_KERNEL")) {
-    if (!strcmp(k, "r28")) e->rsa_kernel = 28;
-    if (!strcmp(k, "r32")) e->rsa_kernel = 32;
-    if (!strcmp(k, "r32sq")) e->rsa_kernel = 33;       // radix 2^32 with the dedicated squaring (the default for 2048-bit moduli)
-  }
-  if (const char* t = getenv("BFTQ_RSA_T")) {
-    int v = atoi(t);
-    if (v == 4 || v == 8) e->rsa_t = v;
-  }
   if (const char* v = getenv("BFTQ_STRICT_RANGE")) if (atoi(v) > 0) e->packer_flags |= BFTQ_F_STRICT_RANGE;
   numa_probe(e);
   e->pool.on_start = [e] { numa_bind_this_thread(e); };

@@ -97,7 +97,7 @@ __device__ __forceinline__ void widen(const uint32_t (&a)[8], uint32_t (&o)[16],
 template <int W>
 __device__ __forceinline__ void mmul(uint32_t (&out)[W], const uint32_t (&a)[W], const uint32_t (&b)[W], const uint32_t (&n)[W], const uint32_t n0inv,
                                      const int r, const int gbase) {
-  r32::mont_mul<W, false, true>(out, a, b, n, n0inv, r, gbase);
+  r32::mont_mul<W, true>(out, a, b, n, n0inv, r, gbase);
 }
 
 // The number 1 in the W = 8 layout.  Recomputed from %laneid at each use (volatile asm): kept live across the exponent

@@ -208,7 +208,7 @@ __device__ __forceinline__ void mont_finish(uint32_t (&out)[W], Acc<W>& A, const
 // out = a * b * R^-1 mod n with R = 2^(128 W), out < R ("almost Montgomery").  a, b < R as W limbs/lane.
 // owners < T stops after that many owner steps: out == a * b' * 2^(-32 W owners) (mod n) with b' the owners' low lanes of b, out < R
 // and, for a < n, out < 2n (K1's final check, one or two owner steps).  All 32 lanes of the warp must call this together.
-template <int W, bool STEP_SYNC = false, bool CT = false>
+template <int W, bool CT = false>
 __device__ __forceinline__ void mont_mul(uint32_t (&out)[W], const uint32_t (&a)[W], const uint32_t (&b)[W],
                                          const uint32_t (&n)[W], const uint32_t n0inv, const int r, const int gbase,
                                          const int owners = T) {
@@ -219,14 +219,9 @@ __device__ __forceinline__ void mont_mul(uint32_t (&out)[W], const uint32_t (&a)
   for (int k = 0; k < W + 2; k++) A.O[k] = 0u;
   uint32_t cin = 0u;      // 1-bit carry pending at position 0
   uint32_t Z = 0u;        // odd-side limb pending at position 0 (the upper half of the O pair the shift cut)
-#ifndef BFTQ_MUL_UNROLL
-#define BFTQ_MUL_UNROLL 1
-#endif
-  constexpr int kMulUnroll = BFTQ_MUL_UNROLL;      // owner steps per loop body (code size x this)
-#pragma unroll kMulUnroll
+#pragma unroll 1
   for (int owner = 0; owner < T; owner++) {
-    if (owner == owners) break;                 // a full trip count keeps BFTQ_MUL_UNROLL free of remainder copies
-    if (STEP_SYNC) __syncthreads();             // keep the block's warps in phase (see BFTQ_K1_SYNC)
+    if (owner == owners) break;                 // a constant trip count with an early exit: with the default owners = T (K5, K6a) the test folds away
     const int src = gbase + owner;
 #pragma unroll
     for (int jj = 0; jj < W; jj += 2) {
@@ -330,38 +325,29 @@ struct RsaKey32 {               // per key, radix 2^32 little-endian words; c = 
   uint32_t pad;
 };
 
-// In-block barriers that keep the four warps of a block in phase (see the kernel's task loop): 0 = none, 1 = once per
-// task, 2 = after every Montgomery product, 3 = 2 + every owner step.  Warps that drift apart fetch different parts of
-// the hot loop and evict each other from the instruction caches; a barrier per product costs 18 bar.sync per 2.3 M
-// instructions.  Measured on H100 (DESIGN.md §4): 0 loses 10 %, 1 loses 5 %, 3 matches 2.
-#ifndef BFTQ_K1_SYNC
-#define BFTQ_K1_SYNC 2
-#endif
-// 1 = the exponentiation runs as one loop over a three-op program (one squaring and one product instance in the kernel
-// instead of the straight-line form's one squaring and two product instances), which keeps the hot loop small enough
-// for the instruction caches (1 % faster than the straight-line form on H100, DESIGN.md §4).
-#ifndef BFTQ_K1_UNIFIED
-#define BFTQ_K1_UNIFIED 1
-#endif
-// SQ: the squarings of the exponentiation go through mont_sqr (rsa_square_r32.cuh) instead of mont_mul(y, y).
-//
+// Threads per block and blocks per SM: 4 blocks of 4 warps at 128 registers per thread fill an SM's 64 K registers.
+constexpr int kK1Block = 128, kK1MinBlocks = 4;
+
 // The exponentiation never converts s to Montgomery form: it runs the square-and-multiply chain of e on the plain s,
 // every 1 bit below the top one a product with the plain s.  A squaring takes y = s^k R^-(k-1) to s^2k R^-(2k-1) and a
 // product with s to s^(k+1) R^-k, so the chain ends at Y = s^e c with c = R^-(e-1) mod n: 16 squarings and one product
 // for e = 65537.  With EM = H 2^k + L (k = 512, or 1024 for T longer than 63 bytes), s^e == EM (mod n) iff
 // Y == c L + hc (mod n); c L is ONE (or two) owner steps of mont_mul with the key's c * 2^k, and hc = H 2^k c mod n is
 // a per-key constant because H = 00 01 FF..FF does not depend on the digest (RsaKey32, bignum_host.hpp).
-template <int BLOCK, int MIN_BLOCKS, bool SQ>
-__global__ void __launch_bounds__(BLOCK, MIN_BLOCKS)
+// The squarings go through mont_sqr (rsa_square_r32.cuh).
+//
+// The four warps of a block meet at a barrier once per task and after every squaring.  Warps that drift apart fetch
+// different parts of the hot loop and evict each other from the instruction caches; without the barriers the kernel
+// loses 10 % on H100 (DESIGN.md §4).
+__global__ void __launch_bounds__(kK1Block, kK1MinBlocks)
 rsa_verify_r32_kernel(const RsaKey32* __restrict__ keys, const uint32_t nkeys, const uint32_t* __restrict__ key_idx,
                       const uint8_t* __restrict__ sig, const uint8_t* __restrict__ digest, const uint32_t hash_alg,
                       const uint64_t n_items, const uint32_t flags, const uint8_t* __restrict__ pre_status,
                       uint8_t* __restrict__ status) {
   constexpr int W = 16;
   constexpr int kGroupsPerWarp = 32 / T;
-  __shared__ uint32_t y_s[W][BLOCK];
+  __shared__ uint32_t y_s[W][kK1Block];
   __shared__ int nbmax_s;
-  constexpr bool kStepSync = BFTQ_K1_SYNC >= 3;
   const int lane = threadIdx.x & 31;
   const int r = lane & (T - 1);
   const int gbase = lane & ~(T - 1);
@@ -369,16 +355,15 @@ rsa_verify_r32_kernel(const RsaKey32* __restrict__ keys, const uint32_t nkeys, c
   const int dlen = c_hash_prefix[hash_alg].dlen;
   const bool wide = plen + dlen > 63;                        // T and its 00 separator reach above 2^512: split EM at 2^1024
   const int check_owners = wide ? 2 : 1;
-  const uint64_t warp_global = (uint64_t)blockIdx.x * (BLOCK / 32) + (threadIdx.x >> 5);
-  const uint64_t warps_total = (uint64_t)gridDim.x * (BLOCK / 32);
+  const uint64_t warps_total = (uint64_t)gridDim.x * (kK1Block / 32);
   const uint32_t gmask = ((1u << T) - 1u) << gbase;
 
   // The trip count is uniform over the block (a warp whose eight signatures lie behind the end computes on clamped items
-  // and stores nothing), so the warps of a block may meet at barriers: BFTQ_K1_SYNC 1 = once per task, 2 = after every
-  // Montgomery product.  Warps that stay in phase fetch the same instructions at the same time (the hot loop is 15 KB).
-  for (uint64_t bbase = (uint64_t)blockIdx.x * (BLOCK / 32) * kGroupsPerWarp; bbase < n_items; bbase += warps_total * kGroupsPerWarp) {
+  // and stores nothing), so the warps of a block may meet at barriers.  Warps that stay in phase fetch the same
+  // instructions at the same time (the hot loop is 15 KB).
+  for (uint64_t bbase = (uint64_t)blockIdx.x * (kK1Block / 32) * kGroupsPerWarp; bbase < n_items; bbase += warps_total * kGroupsPerWarp) {
     const uint64_t wbase = bbase + (uint64_t)(threadIdx.x >> 5) * kGroupsPerWarp;
-    if (BFTQ_K1_SYNC >= 1) __syncthreads();
+    __syncthreads();
     const uint64_t item_raw = wbase + (uint64_t)(lane / T);
     const bool valid = item_raw < n_items;
     const uint64_t item = valid ? item_raw : (n_items - 1);
@@ -403,24 +388,22 @@ rsa_verify_r32_kernel(const RsaKey32* __restrict__ keys, const uint32_t nkeys, c
     int nbmax = nb;
 #pragma unroll
     for (int o = 16; o >= 1; o >>= 1) nbmax = max(nbmax, __shfl_xor_sync(kFull, nbmax, o));
-    if (BFTQ_K1_SYNC >= 2) {                                 // barriers inside the exponent loop: its trip count must be uniform over the block
-      if (threadIdx.x == 0) nbmax_s = 0;
-      __syncthreads();
-      if (lane == 0) atomicMax(&nbmax_s, nbmax);
-      __syncthreads();
-      nbmax = nbmax_s;
-    }
-#if BFTQ_K1_UNIFIED
+    // barriers inside the exponent loop: its trip count must be uniform over the block
+    if (threadIdx.x == 0) nbmax_s = 0;
+    __syncthreads();
+    if (lane == 0) atomicMax(&nbmax_s, nbmax);
+    __syncthreads();
+    nbmax = nbmax_s;
     // The whole verification as ONE loop over a small program, so that the kernel holds a single instance of the
-    // squaring and a single instance of the general product (the straight-line form below has two products; the
-    // instruction caches hold 32 KB).
+    // squaring and a single instance of the general product (a straight-line chain followed by the check product holds
+    // two; the instruction caches hold 32 KB).
     //   op 1: the squaring of `bit`      op 2: y *= s after the squaring of a 1 bit      op 3: the check product c L
     int bit = nbmax - 2, op = bit >= 0 ? 1 : 3;
 #pragma unroll 1
     for (;;) {
       if (op == 1) {
-        if (SQ) mont_sqr<kStepSync>(t, y, nd, n0inv, r, gbase); else mont_mul<W, kStepSync>(t, y, y, nd, n0inv, r, gbase);
-        if (BFTQ_K1_SYNC >= 2) __syncthreads();              // every warp of the block runs nbmax - 1 squarings
+        mont_sqr(t, y, nd, n0inv, r, gbase);
+        __syncthreads();                                     // every warp of the block runs nbmax - 1 squarings
         if (bit <= nb - 2) {
 #pragma unroll
           for (int j = 0; j < W; j++) y[j] = t[j];
@@ -453,35 +436,6 @@ rsa_verify_r32_kernel(const RsaKey32* __restrict__ keys, const uint32_t nkeys, c
     }
 #pragma unroll
     for (int j = 0; j < W; j++) y[j] = y_s[j][threadIdx.x];
-#else
-#pragma unroll 1
-    for (int bit = nbmax - 2; bit >= 0; bit--) {
-      const bool active = bit <= nb - 2;
-      if (SQ) mont_sqr<kStepSync>(t, y, nd, n0inv, r, gbase); else mont_mul<W, kStepSync>(t, y, y, nd, n0inv, r, gbase);
-      if (BFTQ_K1_SYNC >= 2) __syncthreads();
-      if (active) {
-#pragma unroll
-        for (int j = 0; j < W; j++) y[j] = t[j];
-      }
-      const bool mul = active && ((e >> bit) & 1u);
-      if (__any_sync(kFull, mul)) {
-        uint32_t sx[W];
-#pragma unroll
-        for (int j = 0; j < W; j++) sx[j] = be_word(sp, r * W + j);
-        mont_mul(t, y, sx, nd, n0inv, r, gbase);
-        if (mul) {
-#pragma unroll
-          for (int j = 0; j < W; j++) y[j] = t[j];
-        }
-      }
-    }
-    {
-      uint32_t ca[W], lb[W];
-#pragma unroll
-      for (int j = 0; j < W; j++) { ca[j] = __ldg(&ck[r * W + j]); lb[j] = em_word(r * W + j, dp, plen, dlen, hash_alg); }
-      mont_mul(t, ca, lb, nd, n0inv, r, gbase, check_owners);
-    }
-#endif
     // y = Y < 2^2048 < 2n and t = Q == c L (mod n), Q < 2n.  With D = (Y mod n) - (Q mod n) mod 2^2048, borrow b, and
     // F = hc - D mod 2^2048:  Y == Q + hc (mod n)  iff  F == 0 (b = 0: D = Y - Q in [0, n))  or  F == n (b = 1: D + n - 2^2048
     // = Y - Q + n in (0, n)).

@@ -46,30 +46,27 @@ def test_sass_is_carry_free_imad_wide(built):
         assert wide > 100 and widex == 0, (wide, widex)
 
 
-def test_sass_r32_kernels_resource_guard(built):
-    """The radix-2^32 kernels every headline number comes from (rsa_verify_r32_kernel<128, 4, SQ>): carry-chained
-    IMAD.WIDE.U32.X products, 128 registers (4 blocks x 128 threads per SM), at most a few spilled words, no local
-    arrays, and the unified exponentiation loop: ONE general-product instance (4 owner steps x 2 x 57 chained
-    multiplies = 456) plus, in the squaring variant, ONE squaring instance of two owner steps (2 x 337) - the
-    straight-line form carried five instances (2 326 wide multiplies, 7 440 instructions)."""
+def test_sass_r32_kernel_resource_guard(built):
+    """The radix-2^32 kernel every headline number comes from (rsa_verify_r32_kernel): carry-chained IMAD.WIDE.U32.X
+    products, 128 registers (4 blocks x 128 threads per SM), at most a few spilled words, no local arrays, and the
+    unified exponentiation loop: ONE general-product instance (4 owner steps x 2 x 57 chained multiplies = 456) plus
+    ONE squaring instance of two owner steps (2 x 337) - the straight-line form carried five instances (2 326 wide
+    multiplies, 7 440 instructions)."""
     import subprocess
     so = os.path.join(ROOT, "bftkv_b200", "libbftq.so")
     sass = subprocess.run(["cuobjdump", "-sass", so], capture_output=True, text=True).stdout
     res = subprocess.run(["cuobjdump", "-res-usage", so], capture_output=True, text=True).stdout
-    seen = {}
-    for sq in ("Lb0", "Lb1"):
-        name = "rsa_verify_r32_kernelILi128ELi4E" + sq
-        blk = [b for b in sass.split("Function :") if name in b.split("\n")[0]]
-        assert len(blk) == 1, name
-        widex = len(re.findall(r"IMAD\.WIDE\.U32\.X", blk[0]))
-        instrs = len(re.findall(r"/\*[0-9a-f]{4,5}\*/\s+\S", blk[0]))
-        assert 800 < widex < 1400 and instrs < 5600, (name, widex, instrs)
-        m = re.search(r"Function [^\n]*" + name + r"[^\n]*\n\s*REG:(\d+) STACK:(\d+) SHARED:(\d+) LOCAL:(\d+)", res)
-        assert m, name
-        regs, stack, shared, local = map(int, m.groups())
-        assert regs <= 128 and stack <= 64 and local == 0 and shared <= 16384, (name, regs, stack, shared, local)
-        seen[sq] = widex
-    assert seen["Lb0"] == 2 * 456 and seen["Lb1"] == 456 + 2 * 337, seen       # mont_mul twice (as squaring and as product) / mont_mul + mont_sqr x 2 owner steps
+    name = "rsa_verify_r32_kernel"
+    blk = [b for b in sass.split("Function :") if name in b.split("\n")[0]]
+    assert len(blk) == 1, len(blk)
+    widex = len(re.findall(r"IMAD\.WIDE\.U32\.X", blk[0]))
+    instrs = len(re.findall(r"/\*[0-9a-f]{4,5}\*/\s+\S", blk[0]))
+    assert 800 < widex < 1400 and instrs < 5600, (widex, instrs)
+    m = re.search(r"Function [^\n]*" + name + r"[^\n]*\n\s*REG:(\d+) STACK:(\d+) SHARED:(\d+) LOCAL:(\d+)", res)
+    assert m
+    regs, stack, shared, local = map(int, m.groups())
+    assert regs <= 128 and stack <= 64 and local == 0 and shared <= 16384, (regs, stack, shared, local)
+    assert widex == 456 + 2 * 337, widex       # mont_mul + mont_sqr x 2 owner steps
 
 
 def test_sass_int_peak_loop_is_wide_multiplies_only(built):

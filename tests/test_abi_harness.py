@@ -13,16 +13,16 @@ from bftkv_b200 import workload
 from oracle import packet_oracle
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EXE = os.path.join(ROOT, "tests", "harness", "abi_smoke")
 SRC = os.path.join(ROOT, "tests", "harness", "abi_smoke.c")
 
 
-def build_harness():
-    deps = [SRC, os.path.join(ROOT, "include", "bftq.h")]
-    if not os.path.exists(EXE) or os.path.getmtime(EXE) < max(os.path.getmtime(d) for d in deps):
-        subprocess.check_call(["gcc", "-std=c11", "-Wall", "-Wextra", "-Werror", "-O1", "-I" + os.path.join(ROOT, "include"), "-o", EXE, SRC,
-                               "-L" + os.path.join(ROOT, "bftkv_b200"), "-lbftq", "-Wl,-rpath," + os.path.join(ROOT, "bftkv_b200")])
-    return EXE
+@pytest.fixture(scope="session")
+def harness_exe(built, tmp_path_factory):
+    """The harness, built once per session into a temporary directory: the tree may not be writable by the test user."""
+    exe = str(tmp_path_factory.mktemp("harness") / "abi_smoke")
+    subprocess.check_call(["gcc", "-std=c11", "-Wall", "-Wextra", "-Werror", "-O1", "-I" + os.path.join(ROOT, "include"), "-o", exe, SRC,
+                           "-L" + os.path.join(ROOT, "bftkv_b200"), "-lbftq", "-Wl,-rpath," + os.path.join(ROOT, "bftkv_b200")])
+    return exe
 
 
 def u64(v):
@@ -64,12 +64,11 @@ def write_fixture(path):
     open(path, "wb").write(b"".join(out))
 
 
-def test_header_compiles_as_c_and_fails_loudly_without_gpu(built, tmp_path):
+def test_header_compiles_as_c_and_fails_loudly_without_gpu(harness_exe, tmp_path):
     import torch
-    exe = build_harness()
     fx = str(tmp_path / "fixture.bin")
     write_fixture(fx)
-    r = subprocess.run([exe, fx], capture_output=True, text=True)
+    r = subprocess.run([harness_exe, fx], capture_output=True, text=True)
     if not torch.cuda.is_available():
         assert r.returncode == 77, (r.returncode, r.stderr)        # BFTQ_ERR_NO_DEVICE: there is no CPU fallback
     else:
@@ -77,10 +76,9 @@ def test_header_compiles_as_c_and_fails_loudly_without_gpu(built, tmp_path):
 
 
 @pytest.mark.gpu
-def test_c_harness_drives_the_shim_sequence(built, tmp_path):
-    exe = build_harness()
+def test_c_harness_drives_the_shim_sequence(harness_exe, tmp_path):
     fx = str(tmp_path / "fixture.bin")
     write_fixture(fx)
-    r = subprocess.run([exe, fx], capture_output=True, text=True)
+    r = subprocess.run([harness_exe, fx], capture_output=True, text=True)
     assert r.returncode == 0, r.stderr + r.stdout
     assert "abi_smoke ok" in r.stdout

@@ -21,24 +21,18 @@ def batch64k():
     return workload.make_verify_batch(65536, n_keys=16)      # BASELINE config 2
 
 
-def _engine_with(keys, t=None):
-    if t is not None:
-        os.environ["BFTQ_RSA_T"] = str(t)
-    try:
-        e = Engine(0)
-    finally:
-        os.environ.pop("BFTQ_RSA_T", None)
+def _engine_with(keys):
+    e = Engine(0)
     e.register_rsa_keys([k["n"] for k in keys], [k["e"] for k in keys])
     return e
 
 
-@pytest.mark.parametrize("t", [4, 8])
-def test_config2_full_batch_bit_exact(batch64k, built, t):
+def test_config2_full_batch_bit_exact(batch64k, built):
     w = batch64k
     ns, es = [k["n"] for k in w["keys"]], [k["e"] for k in w["keys"]]
     ref = c_oracle.rsa_verify_batch(ns, es, w["key_idx"], w["sig"], w["digest"], threads=NCPU)
     assert np.array_equal(ref, w["expect"])
-    e = _engine_with(w["keys"], t)
+    e = _engine_with(w["keys"])
     got = e.rsa_verify_batch(w["key_idx"], w["sig"], w["digest"])
     assert np.array_equal(got, ref)
     assert (got == 0).sum() > 60000 and (got == 1).sum() > 300 and (got == 4).sum() > 20
@@ -125,10 +119,9 @@ def test_other_exponents_and_key_sizes(built):
         sig[i, int(rng.integers(1, 256))] ^= 0x40
     ref = c_oracle.rsa_verify_batch(ns, es, kidx, sig, dig, threads=NCPU)
     assert set(ref[~flip]) == {0} and set(ref[flip]) == {1}
-    for t in (4, 8):
-        e = _engine_with(keys, t)
-        assert np.array_equal(e.rsa_verify_batch(kidx, sig, dig), ref)
-        e.close()
+    e = _engine_with(keys)
+    assert np.array_equal(e.rsa_verify_batch(kidx, sig, dig), ref)
+    e.close()
     # an even public exponent cannot come from a valid key, but x/crypto parses it and
     # big.Int.Exp computes it: the decision must still equal s^e mod n == EM.
     keys2 = [{"n": fix[0]["n"], "e": 65536}, {"n": fix[1]["n"], "e": 2}, {"n": fix[2]["n"], "e": 1}]
@@ -138,10 +131,9 @@ def test_other_exponents_and_key_sizes(built):
     dig2 = np.repeat(dig[:1], 4, axis=0).copy()
     ref2 = c_oracle.rsa_verify_batch([k["n"] for k in keys2], [k["e"] for k in keys2], kidx2, sig2, dig2)
     assert ref2.tolist() == [1, 1, 0, 1]
-    for t in (4, 8):
-        e = _engine_with(keys2, t)
-        assert np.array_equal(e.rsa_verify_batch(kidx2, sig2, dig2), ref2)
-        e.close()
+    e = _engine_with(keys2)
+    assert np.array_equal(e.rsa_verify_batch(kidx2, sig2, dig2), ref2)
+    e.close()
 
 
 def test_gpg_golden_signatures(golden, built):
@@ -215,19 +207,12 @@ def test_roundtrip_property_fresh_keys(built):
     e.close()
 
 
-@pytest.mark.parametrize("variant", ["r32", "r32sq"])
-def test_r32_kernel_variants_bit_exact(batch64k, built, variant):
-    """Both radix-2^32 kernels — squarings through mont_sqr (rsa_square_r32.cuh, the default; emulated limb for limb by
-    tools/emu_sq.py) and through the general product mont_mul(y, y) (BFTQ_RSA_KERNEL=r32) — against the oracle on
-    config 2, ragged sizes and the edge values of s."""
+def test_r32_kernel_bit_exact(batch64k, built):
+    """The radix-2^32 kernel (squarings through mont_sqr, rsa_square_r32.cuh, emulated limb for limb by tools/emu_sq.py)
+    against the oracle on config 2, ragged sizes and the edge values of s."""
     w = batch64k
     ns, es = [k["n"] for k in w["keys"]], [k["e"] for k in w["keys"]]
-    os.environ["BFTQ_RSA_KERNEL"] = variant
-    try:
-        e = Engine(0)
-    finally:
-        del os.environ["BFTQ_RSA_KERNEL"]
-    e.register_rsa_keys(ns, es)
+    e = _engine_with(w["keys"])
     ref = c_oracle.rsa_verify_batch(ns, es, w["key_idx"], w["sig"], w["digest"], threads=NCPU)
     got = e.rsa_verify_batch(w["key_idx"], w["sig"], w["digest"])
     assert np.array_equal(got, ref)
