@@ -16,8 +16,9 @@
 // unchanged; no shared memory, no second pass.
 // The doubled operand is the lane-local a2 = 2 * A_X (17 limbs, a2[16] = the bit shifted out): a row uses a2[k] for
 // k >= j + 2, two patched limbs at k = j and j + 1, and the bit a2[16] as an addend of the chain's first carry limb
-// (free).  The pending 1-bit carry `cin`, which mont_mul feeds into the a x b chain at slot 0, enters with the n x q0
-// chain here (the a x a chains no longer start at slot 0).  tools/emu_sq.py emulates this file limb for limb.
+// (free).  Unlike mont_mul, a step leaves no pending limb at position 0: the next step's position 0 is folded into one
+// limb at once, and the 1-bit carry out of it waits at position 1 and enters with the n x q1 chain.  tools/emu_sq.py
+// emulates this file limb for limb.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -44,11 +45,19 @@ __device__ __forceinline__ void chain_n(uint32_t* p, uint32_t& c0, uint32_t& c1,
   for (int i = 1; i < N; i++) mad_pair_next(p[2 * i], p[2 * i + 1], x[2 * i], m);
   asm volatile("addc.cc.u32 %0, %0, %2; addc.u32 %1, %1, 0;" : "+r"(c0), "+r"(c1) : "r"(t));
 }
+// The same with one carry limb, for a chain whose carry lands on position 18, which never overflows (see sqr_iter).
+template <int N>
+__device__ __forceinline__ void chain_n1(uint32_t* p, uint32_t& c, const uint32_t* x, const uint32_t m) {
+  mad_pair_first(p[0], p[1], x[0], m);
+#pragma unroll
+  for (int i = 1; i < N; i++) mad_pair_next(p[2 * i], p[2 * i + 1], x[2 * i], m);
+  asm volatile("addc.u32 %0, %0, 0;" : "+r"(c));
+}
 
 // One iteration of the squaring loop: the rows JJ and JJ + 1 of owner lane `owner` (JJ even, compile-time), then the
 // reduction by two limbs exactly as in mont_mul.
 template <int JJ>
-__device__ __forceinline__ void sqr_iter(Acc<16>& A, uint32_t& cin, uint32_t& Z, const uint32_t (&a2)[17], const uint32_t (&n)[16],
+__device__ __forceinline__ void sqr_iter(Acc<16>& A, uint32_t& cy1, const uint32_t (&a2)[17], const uint32_t (&n)[16],
                                          const uint32_t n0inv, const int r, const int gbase, const int owner) {
   constexpr int W = 16;
   const uint32_t lt1 = r < owner ? ~1u : 0u, nm = r < owner ? ~0u : ~1u, eqm = r == owner ? ~0u : 0u;
@@ -73,35 +82,40 @@ __device__ __forceinline__ void sqr_iter(Acc<16>& A, uint32_t& cin, uint32_t& Z,
   const uint32_t t1 = (0u - top1) & b1;
   // ---- offset 0 ---------------------------------------------------------------------------------------------
   chain_n<(W - JJ) / 2>(A.E + JJ, A.E[W], A.E[W + 1], m0 + JJ, b0, t0);                 // even limbs >= JJ      -> E pairs (k, k+1)
-  uint32_t q0 = (A.E[0] + Z + cin) * n0inv;
+  uint32_t q0 = A.E[0] * n0inv;
   q0 = __shfl_sync(kFull, q0, gbase);
   chain_n<(W - JJ) / 2>(A.O + JJ, A.O[W], A.O[W + 1], m0 + JJ + 1, b0, 0u);             // odd limbs  >= JJ + 1  -> O pairs (k-1, k)
   chain_n<(W - JJ - 2) / 2>(A.O + JJ + 2, A.O[W], A.O[W + 1], m1 + JJ + 2, b1, t1);     // even limbs >= JJ + 2  -> O pairs (k, k+1)
-  chain_n<(W - JJ) / 2>(A.E + JJ + 2, A.E[W + 2], A.E[W + 3], m1 + JJ + 1, b1, 0u);     // odd limbs  >= JJ + 1  -> E pairs (k+1, k+2)
-  mac_off0_even(A, n, q0, cin);
+  chain_n1<(W - JJ) / 2>(A.E + JJ + 2, A.O[W + 1], m1 + JJ + 1, b1);                       // odd limbs  >= JJ + 1  -> E pairs (k+1, k+2)
+  mac_off0_even_nocin(A, n, q0);
   mac_off0_odd(A, n, q0);
   // ---- offset 1 ---------------------------------------------------------------------------------------------
-  const uint64_t s0 = (uint64_t)A.E[0] + Z;
-  const uint32_t p0 = (uint32_t)s0, c0 = (uint32_t)(s0 >> 32);
-  uint32_t q1 = (A.E[1] + A.O[0] + c0) * n0inv;
+  uint32_t q1 = (A.E[1] + A.O[0] + cy1) * n0inv;
   q1 = __shfl_sync(kFull, q1, gbase);
-  mac_off1_even(A, n, q1);
-  mac_off1_odd(A, n, q1);
-  const uint64_t s1 = (uint64_t)A.E[1] + A.O[0] + c0;
-  const uint32_t p1 = (uint32_t)s1;
-  cin = (uint32_t)(s1 >> 32);
-  Z = A.O[1];
+  Chain<W>::run_cin(A.O, A.O[W], A.O[W + 1], n, q1, cy1);                              // mac_off1_even, cy1 enters at position 1
+  chain_n1<W / 2>(A.E + 2, A.O[W + 1], n + 1, q1);                                      // mac_off1_odd, carry -> O[W + 1]
+  // positions 0 and 1 leave the lane (lane 0's are zero, the others' go to the lane below).  Position 2, the next step's
+  // position 0, becomes one limb: E[2] + O[1] + the carry out of position 1, whose own carry cy1 waits at position 1.
+  const uint32_t p0 = A.E[0];
+  uint32_t p1, e0;
+  asm("add.cc.u32 %0, %3, %4; addc.cc.u32 %1, %5, %6; addc.u32 %2, 0, 0;"
+      : "=r"(p1), "=r"(e0), "=r"(cy1) : "r"(A.E[1]), "r"(A.O[0]), "r"(A.E[2]), "r"(A.O[1]));
   uint32_t r0 = __shfl_down_sync(kFull, p0, 1, T);
   uint32_t r1 = __shfl_down_sync(kFull, p1, 1, T);
   if (r == T - 1) { r0 = 0u; r1 = 0u; }
+  // Shift down two limbs.  E and O keep 16 limbs each plus two carry limbs that are zero when a step starts; E[W + 2]
+  // and E[W + 3] are never used here.  A lane's accumulated value stays below 2^515 between steps and below 2^579 within
+  // one, so position 18 (O[W + 1], where the chains into E[W]..E[W + 1] put their carry, one instruction each) holds a
+  // few units and position 19 nothing, and after the shift position 16 (O[W - 1]) takes the carry of the two limbs from
+  // the lane above without overflowing (tools/emu_sq.py asserts both).
 #pragma unroll
-  for (int k = 0; k < W + 2; k++) A.E[k] = A.E[k + 2];
-  A.E[W + 2] = 0u; A.E[W + 3] = 0u;
+  for (int k = 1; k < W; k++) A.E[k] = A.E[k + 2];
+  A.E[0] = e0; A.E[W] = 0u; A.E[W + 1] = 0u;
 #pragma unroll
   for (int k = 0; k < W; k++) A.O[k] = A.O[k + 2];
   A.O[W] = 0u; A.O[W + 1] = 0u;
-  asm volatile("add.cc.u32 %0, %0, %4; addc.cc.u32 %1, %1, %5; addc.cc.u32 %2, %2, 0; addc.u32 %3, %3, 0;"
-               : "+r"(A.E[W - 2]), "+r"(A.E[W - 1]), "+r"(A.E[W]), "+r"(A.E[W + 1]) : "r"(r0), "r"(r1));
+  asm volatile("add.cc.u32 %0, %0, %3; addc.cc.u32 %1, %1, %4; addc.u32 %2, %2, 0;"
+               : "+r"(A.E[W - 2]), "+r"(A.E[W - 1]), "+r"(A.O[W - 1]) : "r"(r0), "r"(r1));
 }
 
 // out = a * a * R^-1 mod n, out < R ("almost Montgomery"), R = 2^2048.  All 32 lanes of the warp call this together.
@@ -118,20 +132,24 @@ __device__ __forceinline__ void mont_sqr(uint32_t (&out)[16], const uint32_t (&a
   for (int k = 0; k < W + 4; k++) A.E[k] = 0u;
 #pragma unroll
   for (int k = 0; k < W + 2; k++) A.O[k] = 0u;
-  uint32_t cin = 0u, Z = 0u;
+  uint32_t cy1 = 0u;            // 1-bit carry pending at position 1
   // two owner steps per loop body: half the back-edge register moves of one step (2 % faster on H100, DESIGN.md §4)
 #pragma unroll 2
   for (int owner = 0; owner < T; owner++) {
-    sqr_iter<0>(A, cin, Z, a2, n, n0inv, r, gbase, owner);
-    sqr_iter<2>(A, cin, Z, a2, n, n0inv, r, gbase, owner);
-    sqr_iter<4>(A, cin, Z, a2, n, n0inv, r, gbase, owner);
-    sqr_iter<6>(A, cin, Z, a2, n, n0inv, r, gbase, owner);
-    sqr_iter<8>(A, cin, Z, a2, n, n0inv, r, gbase, owner);
-    sqr_iter<10>(A, cin, Z, a2, n, n0inv, r, gbase, owner);
-    sqr_iter<12>(A, cin, Z, a2, n, n0inv, r, gbase, owner);
-    sqr_iter<14>(A, cin, Z, a2, n, n0inv, r, gbase, owner);
+    sqr_iter<0>(A, cy1, a2, n, n0inv, r, gbase, owner);
+    sqr_iter<2>(A, cy1, a2, n, n0inv, r, gbase, owner);
+    sqr_iter<4>(A, cy1, a2, n, n0inv, r, gbase, owner);
+    sqr_iter<6>(A, cy1, a2, n, n0inv, r, gbase, owner);
+    sqr_iter<8>(A, cy1, a2, n, n0inv, r, gbase, owner);
+    sqr_iter<10>(A, cy1, a2, n, n0inv, r, gbase, owner);
+    sqr_iter<12>(A, cy1, a2, n, n0inv, r, gbase, owner);
+    sqr_iter<14>(A, cy1, a2, n, n0inv, r, gbase, owner);
   }
-  mont_finish(out, A, cin, Z, n, r, gbase);
+  // cy1 into O (position 1 on): the value bound keeps the ripple inside O[W - 1]
+  asm volatile("add.cc.u32 %0, %0, %1;" : "+r"(A.O[0]) : "r"(cy1));
+#pragma unroll
+  for (int k = 1; k < W; k++) asm volatile("addc.cc.u32 %0, %0, 0;" : "+r"(A.O[k]));
+  mont_finish(out, A, 0u, 0u, n, r, gbase);
 }
 
 }  // namespace r32

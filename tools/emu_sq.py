@@ -10,6 +10,10 @@ in row i of lane M, never both), every lane multiplies 16 - j (+/- 1) limbs in r
 shrink together: 136 limb products per lane and step instead of 256.
 The doubled operand is the lane-local a2 = 2 * A_X (17 limbs, a2[16] = carry bit); a row uses a2[k] for k >= j + 2,
 two patched limbs at k = j, j + 1, and the bit a2[16] as an addend of the chain's first carry limb.
+The chains into the E pairs up to (16, 17) put their carry on position 18, which is O[17] (`end` asserts that it never
+overflows), and the limbs handed down by the lane above carry into position 16 after the shift, which is O[15].
+No pending limb is kept at position 0: a step ends by folding the next step's position 0 into one limb, and the carry out
+of it (cy1) waits at position 1 and enters with the n x q1 chain.
 """
 import random
 B = 1 << 32; T = 4; W = 16; M32 = B - 1
@@ -59,7 +63,7 @@ def montsqr_acc(a, n, n0inv):
     for r in range(T):
         v = sum(al[r][k] << (32 * k) for k in range(W)) * 2
         a2.append([(v >> (32 * k)) & M32 for k in range(17)])
-    E = [[0] * 20 for _ in range(T)]; O = [[0] * 18 for _ in range(T)]; cin = [0] * T; Z = [0] * T
+    E = [[0] * 20 for _ in range(T)]; O = [[0] * 18 for _ in range(T)]; cy1 = [0] * T
     nprod = 0
     for Y in range(T):
         for jj in range(0, W, 2):
@@ -75,30 +79,36 @@ def montsqr_acc(a, n, n0inv):
             for r in range(T):
                 m0, _ = ops0[r]
                 c = chain(E[r], [(k, k) for k in ev0], m0, b0); end(E[r], 16, c, 2, add=m0[16] * b0)
-            q0 = (((E[0][0] + Z[0] + cin[0]) & M32) * n0inv) & M32      # the pending carry enters with the n x q0 chain (slot 0)
+            q0 = ((E[0][0] & M32) * n0inv) & M32
             for r in range(T):
                 m0, _ = ops0[r]; m1, _ = ops1[r]
                 c = chain(O[r], [(k - 1, k) for k in od0], m0, b0); end(O[r], 16, c, 2)
                 c = chain(O[r], [(k, k) for k in ev1], m1, b1); end(O[r], 16, c, 2, add=m1[16] * b1)
-                c = chain(E[r], [(k + 1, k) for k in od1], m1, b1); end(E[r], 18, c, 2)
-                c = chain(E[r], [(k, k) for k in range(0, W, 2)], nl[r], q0, cin[r]); end(E[r], 16, c, 2)
+                c = chain(E[r], [(k + 1, k) for k in od1], m1, b1); end(O[r], 17, c, 1)     # position 18 = O[17]
+                c = chain(E[r], [(k, k) for k in range(0, W, 2)], nl[r], q0); end(E[r], 16, c, 2)
                 c = chain(O[r], [(k - 1, k) for k in range(1, W, 2)], nl[r], q0); end(O[r], 16, c, 2)
-            s0 = [E[r][0] + Z[r] for r in range(T)]; c0 = [x >> 32 for x in s0]; p0 = [x & M32 for x in s0]
-            q1 = (((E[0][1] + O[0][0] + c0[0]) & M32) * n0inv) & M32
-            p1 = [0] * T
+            p0 = [E[r][0] for r in range(T)]
+            q1 = (((E[0][1] + O[0][0] + cy1[0]) & M32) * n0inv) & M32
+            p1 = [0] * T; e0 = [0] * T
             for r in range(T):
-                c = chain(O[r], [(k, k) for k in range(0, W, 2)], nl[r], q1); end(O[r], 16, c, 2)
-                c = chain(E[r], [(k + 1, k) for k in range(1, W, 2)], nl[r], q1); end(E[r], 18, c, 2)
-                s = E[r][1] + O[r][0] + c0[r]; p1[r] = s & M32; cin[r] = s >> 32
+                c = chain(O[r], [(k, k) for k in range(0, W, 2)], nl[r], q1, cy1[r]); end(O[r], 16, c, 2)   # cy1 enters at position 1
+                c = chain(E[r], [(k + 1, k) for k in range(1, W, 2)], nl[r], q1); end(O[r], 17, c, 1)
+                s = E[r][1] + O[r][0]; p1[r] = s & M32
+                s = E[r][2] + O[r][1] + (s >> 32); e0[r] = s & M32; cy1[r] = s >> 32     # the next step's position 0, one limb
             assert p0[0] == 0 and p1[0] == 0
             for r in range(T):
                 r0 = p0[r + 1] if r < T - 1 else 0; r1 = p1[r + 1] if r < T - 1 else 0
-                Z[r] = O[r][1]
-                E[r] = E[r][2:] + [0, 0]; O[r] = O[r][2:] + [0, 0]
-                v = E[r][14] + (E[r][15] << 32) + (E[r][16] << 64) + (E[r][17] << 96) + r0 + (r1 << 32)
-                E[r][14] = v & M32; E[r][15] = (v >> 32) & M32; E[r][16] = (v >> 64) & M32; E[r][17] = (v >> 96) & M32
-                assert v >> 128 == 0
-    return E, O, Z, cin, nprod
+                assert E[r][18] == 0 and E[r][19] == 0            # the kernel keeps no limbs above E[17]
+                # E and O keep 16 limbs each plus two carry limbs that start every step at zero; position 16 is O[15]
+                E[r] = [e0[r]] + E[r][3:18] + [0, 0, 0, 0]; O[r] = O[r][2:] + [0, 0]
+                v = E[r][14] + (E[r][15] << 32) + (O[r][15] << 64) + r0 + (r1 << 32)
+                E[r][14] = v & M32; E[r][15] = (v >> 32) & M32; O[r][15] = (v >> 64) & M32
+                assert v >> 96 == 0
+    for r in range(T):                                    # mont_sqr's tail: cy1 rippled into O (position 1 on)
+        v = sum(O[r][k] << (32 * k) for k in range(W)) + cy1[r]
+        assert v >> (32 * W) == 0
+        O[r][:W] = [(v >> (32 * k)) & M32 for k in range(W)]
+    return E, O, [0] * T, [0] * T, nprod
 
 
 def montsqr_emu(a, n, n0inv):
