@@ -29,7 +29,6 @@
 #include <deque>
 #include <functional>
 #include <map>
-#include <tuple>
 #include <memory>
 #include <thread>
 #include <mutex>
@@ -53,6 +52,22 @@ int fail(int code, const std::string& msg) {
     if (_e != cudaSuccess)                                                                    \
       return fail(BFTQ_ERR_CUDA, std::string(#call) + ": " + cudaGetErrorString(_e));         \
   } while (0)
+
+// Tunables from the environment (INTEGRATION.md lists them).  Each caller decides WHEN its variable is read: a function
+// static reads it once per process, a plain call on every use.
+bool env_set(const char* name) { return getenv(name) != nullptr; }
+// A positive number, else the default.
+uint64_t env_u64(const char* name, uint64_t dflt) {
+  const char* v = getenv(name);
+  const long long x = v ? atoll(v) : 0;
+  return x > 0 ? (uint64_t)x : dflt;
+}
+// A switch that is on by default stays on unless set to 0; one that is off by default stays off unless set to a positive number.
+bool env_on(const char* name, bool dflt) {
+  const char* v = getenv(name);
+  if (!v) return dflt;
+  return dflt ? atoi(v) != 0 : atoi(v) > 0;
+}
 
 using namespace bftq::hostbig;
 
@@ -249,7 +264,7 @@ void scratch_release(bftq_engine* e, void* p, size_t bytes) {
 
 void numa_probe(bftq_engine* e) {
   e->numa_valid = false;
-  if (const char* v = getenv("BFTQ_NUMA_BIND")) if (atoi(v) == 0) return;
+  if (!env_on("BFTQ_NUMA_BIND", true)) return;
   char bdf[32] = {0};
   if (cudaDeviceGetPCIBusId(bdf, sizeof(bdf), e->device) != cudaSuccess) { cudaGetLastError(); return; }
   for (char* c = bdf; *c; c++) *c = (char)tolower(*c);
@@ -460,6 +475,27 @@ class Arena {
   size_t total_ = 0;
 };
 
+// A host batch travels as chunks through a ring of four staging slots, one stream each: the copies of chunk c + 1 run
+// under the kernels of chunk c, and kernels of neighbouring chunks run out of phase.
+struct ArenaRing {
+  bftq_engine* e;
+  std::unique_ptr<Arena> slots[4];
+  uint64_t n = 0;
+  Arena& next(int& rc) {                       // the oldest chunk is finished (rc: its result) and a fresh arena takes its place
+    std::unique_ptr<Arena>& slot = slots[n++ % 4];
+    rc = slot ? slot->finish() : (int)BFTQ_OK;
+    slot.reset(new Arena(e));
+    return *slot;
+  }
+  int drain(int rc) {                          // finishes every chunk still in flight; the first error (rc included) wins
+    for (auto& slot : slots) if (slot) { const int r2 = slot->finish(); if (!rc) rc = r2; slot.reset(); }
+    return rc;
+  }
+};
+// Items per chunk of such a batch (tools/e2e_experiment.py compares one unchunked call with four 16384-item pieces in
+// flight); BFTQ_HOST_CHUNK overrides, read once per process.
+uint64_t host_chunk() { static const uint64_t n = env_u64("BFTQ_HOST_CHUNK", 16384); return n; }
+
 // The key table a launch indexes: a consistent snapshot of the engine's published table (taken under e->mu), or the
 // table of one call (keys presented with the call).
 struct KeyView {
@@ -599,7 +635,7 @@ int bftq_init(int device, bftq_engine** out) {
   auto* e = new bftq_engine();
   e->device = device;
   e->sm_count = prop.multiProcessorCount;
-  if (const char* v = getenv("BFTQ_STRICT_RANGE")) if (atoi(v) > 0) e->packer_flags |= BFTQ_F_STRICT_RANGE;
+  if (env_on("BFTQ_STRICT_RANGE", false)) e->packer_flags |= BFTQ_F_STRICT_RANGE;
   numa_probe(e);
   e->pool.on_start = [e] { numa_bind_this_thread(e); };
   *out = e;
@@ -819,21 +855,16 @@ int bftq_rsa_verify_batch_k(bftq_engine* e, uint32_t key_bytes, const uint32_t* 
   if (n_items == 0) return BFTQ_OK;
   const KeyView kv = global_keys(e);
   if (!kv.d_keys) return fail(BFTQ_ERR_INVALID_ARG, "no keys registered");
-  // Large batches are cut into chunks that travel through a ring of staging slots (one stream each): the copy of
-  // chunk c+1 runs under the kernel of chunk c, and kernels of neighbouring chunks run out of phase
-  // (tools/e2e_experiment.py compares one unchunked call with four 16384-item pieces in flight).
-  static const uint64_t kChunk = [] { const char* v = getenv("BFTQ_HOST_CHUNK"); const long long c = v ? atoll(v) : 16384; return (uint64_t)(c > 0 ? c : 16384); }();
-  constexpr int kDepth = 4;
+  // Large batches are cut into equal chunks of about host_chunk() items (ArenaRing).
+  const uint64_t kChunk = host_chunk();
   const uint64_t n_chunks = n_items <= kChunk + kChunk / 2 ? 1 : (n_items + kChunk - 1) / kChunk;
   const uint64_t per = (n_items + n_chunks - 1) / n_chunks;
-  std::unique_ptr<Arena> ring[kDepth];
+  ArenaRing ring{e};
   int rc = BFTQ_OK;
   for (uint64_t c = 0; c < n_chunks && rc == BFTQ_OK; c++) {
     const uint64_t lo = c * per, cnt = std::min(per, n_items - lo);
-    std::unique_ptr<Arena>& slot = ring[c % kDepth];
-    if (slot) { rc = slot->finish(); slot.reset(); if (rc) break; }
-    slot.reset(new Arena(e));
-    Arena& a = *slot;
+    Arena& a = ring.next(rc);
+    if (rc) break;
     uint8_t *d_sig, *d_dig, *d_st; uint32_t* d_idx;
     a.in(&d_sig, sig_be + lo * key_bytes, (size_t)cnt * key_bytes);
     a.in(&d_dig, digest + lo * dlen, (size_t)cnt * dlen);
@@ -845,8 +876,7 @@ int bftq_rsa_verify_batch_k(bftq_engine* e, uint32_t key_bytes, const uint32_t* 
     if (rc) break;
     rc = a.download_async();
   }
-  for (auto& slot : ring) if (slot) { const int r2 = slot->finish(); if (!rc) rc = r2; slot.reset(); }
-  return rc;
+  return ring.drain(rc);
 }
 
 // ---- K1b --------------------------------------------------------------------------------------
@@ -893,8 +923,7 @@ int ed_cache_prepare(bftq_engine* e, const uint8_t* pubkeys, uint32_t n_keys, ui
   }
   if (fresh.size() > max_new) return BFTQ_OK;                  // too few signatures to pay for this many new tables
   if (c.cap_slots == 0) {                                      // first use: the cache itself and the base point's table
-    uint32_t cap = 256;
-    if (const char* v = getenv("BFTQ_ED25519_CACHE_SLOTS")) cap = (uint32_t)std::max(1, atoi(v));
+    const uint32_t cap = (uint32_t)env_u64("BFTQ_ED25519_CACHE_SLOTS", env_set("BFTQ_ED25519_CACHE_SLOTS") ? 1 : 256);   // set: at least one slot
     void *tab = nullptr, *tabB = nullptr, *hdr = nullptr;
     if (cudaMalloc(&tab, (size_t)cap * ed::FxA::entries * sizeof(ed::gea)) != cudaSuccess ||
         cudaMalloc(&tabB, (size_t)ed::FxB::entries * sizeof(ed::gea)) != cudaSuccess ||
@@ -968,7 +997,7 @@ int bftq_ed25519_verify_batch_dev(bftq_engine* e, const uint8_t* pubkeys, uint32
   // about 1 000 such verifications' worth of work once per key and engine (about 100 table-free ones), so a batch may
   // bring one NEW key per 32 signatures; keys that are cached already cost nothing, whatever the batch size.  Batches
   // with more new keys than that (every signature under its own key, say) take the table-free double-and-add kernel.
-  static const bool no_tables = [] { const char* v = getenv("BFTQ_ED25519_TABLES"); return v && atoi(v) == 0; }();
+  static const bool no_tables = !env_on("BFTQ_ED25519_TABLES", true);
   bool tables = !no_tables && n_keys > 0 && n_keys <= 4096;
   int launches = 0;
   if (tables) {
@@ -1232,11 +1261,10 @@ static int verify_tally_host(bftq_engine* e, const bftq_quorum* q, const uint32_
     if (op_off[i + 1] < op_off[i]) return fail(BFTQ_ERR_INVALID_ARG, "op_off must be non-decreasing");
     if (read && op_off[i + 1] - op_off[i] > 32) return fail(BFTQ_ERR_INVALID_ARG, "read tally: more than 32 responders in one operation");
   }
-  static const uint64_t kChunk = [] { const char* v = getenv("BFTQ_HOST_CHUNK"); const long long c = v ? atoll(v) : 16384; return (uint64_t)(c > 0 ? c : 16384); }();
-  constexpr int kDepth = 4;
-  std::unique_ptr<Arena> ring[kDepth];
+  const uint64_t kChunk = host_chunk();
+  ArenaRing ring{e};
   int rc = BFTQ_OK;
-  uint64_t lo = 0, c = 0;
+  uint64_t lo = 0;
   while (lo < n_ops && rc == BFTQ_OK) {
     // chunk [lo, hi): whole operations, about kChunk tuples (at least one operation)
     uint64_t hi = lo + 1;
@@ -1249,10 +1277,8 @@ static int verify_tally_host(bftq_engine* e, const bftq_quorum* q, const uint32_
     }
     const uint64_t t0 = op_off[lo], cnt = op_off[hi] - t0, nops = hi - lo;
     const size_t ni = (size_t)std::max<uint64_t>(cnt, 1);
-    std::unique_ptr<Arena>& slot = ring[c % kDepth];
-    if (slot) { rc = slot->finish(); slot.reset(); if (rc) break; }
-    slot.reset(new Arena(e));
-    Arena& a = *slot;
+    Arena& a = ring.next(rc);
+    if (rc) break;
     uint32_t *d_off, *h_off, *d_idx, *d_val = nullptr, *d_win = nullptr, *d_at = nullptr;
     uint8_t *d_sig, *d_dig, *d_pre = nullptr, *d_st, *d_bits, *d_dec = nullptr; uint64_t* d_ts = nullptr;
     a.in(&d_sig, sig_be + t0 * 256, ni * 256, (size_t)cnt * 256);
@@ -1273,10 +1299,9 @@ static int verify_tally_host(bftq_engine* e, const bftq_quorum* q, const uint32_
                                a.stream());
     if (rc) break;
     rc = a.download_async();
-    lo = hi; c++;
+    lo = hi;
   }
-  for (auto& slot : ring) if (slot) { const int r2 = slot->finish(); if (!rc) rc = r2; slot.reset(); }
-  return rc;
+  return ring.drain(rc);
 }
 
 int bftq_verify_tally_batch(bftq_engine* e, const bftq_quorum* q, const uint32_t* op_off, const uint32_t* key_idx,
