@@ -15,7 +15,13 @@ overflows), and the limbs handed down by the lane above carry into position 16 a
 No pending limb is kept at position 0: a step ends by folding the next step's position 0 into one limb, and the carry out
 of it (cy1) waits at position 1 and enters with the n x q1 chain.
 """
+import os
 import random
+import sys
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from emu_r32 import mont_finish_emu, value  # noqa: E402
+
 B = 1 << 32; T = 4; W = 16; M32 = B - 1
 
 
@@ -122,10 +128,18 @@ def montsqr_emu(a, n, n0inv):
     return tot, nprod
 
 
-if __name__ == "__main__":
-    random.seed(2)
+def mont_sqr_emu(a, n, trace=None):
+    """mont_sqr with its mont_finish (emu_r32.mont_finish_emu, `trace` as there): a^2 R^-1 mod n, < R"""
+    E, O, Z, cin, _ = montsqr_acc(a, n, (-pow(n, -1, B)) % B)
+    return value(mont_finish_emu(E, O, Z, cin, n, W, trace))
+
+
+def check_random(iters=300, seed=2):
+    """random and adversarial squarings (operands R - 1, alternating limbs, single bits; modulus R - 1) against
+    big-int arithmetic; returns the a x a limb products per lane and squaring"""
+    random.seed(seed)
     R = 1 << 2048
-    for it in range(300):
+    for it in range(iters):
         n = random.getrandbits(2048) | (1 << 2047) | 1
         a = random.getrandbits(2048)
         if it % 7 == 0: a = R - 1
@@ -137,4 +151,9 @@ if __name__ == "__main__":
         t, nprod = montsqr_emu(a, n, n0inv)
         assert t == (a * a + ((a * a * (-pow(n, -1, R))) % R) * n) // R, it
         assert t < R + n
+    return nprod
+
+
+if __name__ == "__main__":
+    nprod = check_random()
     print("emulation ok; a x a limb products per lane and squaring:", nprod, "(general product: 1024)")
