@@ -108,6 +108,10 @@ def load():
         "bftq_graph_choose_quorum": (C.c_int, [vp, C.c_int, vp, C.c_uint32, u32p, vp, C.c_uint32, u32p]),
         "bftq_stats": (C.c_int, [vp, C.POINTER(Stats)]),
         "bftq_measure_int_peak": (C.c_int, [vp, C.POINTER(C.c_double)]),
+        "bftq_thrsa_share_create": (C.c_int, [vp, vp, C.c_uint64, C.POINTER(vp)]),
+        "bftq_thrsa_share_destroy": (None, [vp]),
+        "bftq_thrsa_sign_batch": (C.c_int, [vp, vp, C.c_uint32, vp, vp, vp, C.c_uint64, vp, vp, C.c_uint64, vp]),
+        "bftq_thrsa_process_batch": (C.c_int, [vp, C.c_uint32, C.c_uint32, vp, vp, vp, C.c_uint64, vp, vp, vp, vp, vp, C.c_uint64, vp]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(lib, name)       # AttributeError here = header/library mismatch: fail loudly

@@ -412,3 +412,58 @@ def read_responses_batch(kr: "Keyring", qcs, op_off, peer_ids, msgs: Sequence[by
     for k in ("status", "ts", "value_off", "value_len"):
         out[k] = out[k][:n]
     return out
+
+
+ErrInvalidInput = "crypto: invalid input"
+ErrInsufficientNumberOfThresholdSignatures = "crypto: insufficient number of threshold signatures"
+
+
+class ThresholdRSA:
+    """crypto.Threshold for TH_RSA (crypto/threshold/rsa/rsa.go): the server's Sign over registered shares and the client's
+    ProcessResponse, both batched.  A share is the saved parameter (ThresholdInstance's secret without its algo byte)."""
+
+    def __init__(self, engine: Engine):
+        self.engine = engine
+        self._shares = {}
+
+    def register(self, sec: bytes):
+        """Uploads a share once (opt-in: its fragments then live on the device until close())."""
+        if sec not in self._shares:
+            self._shares[sec] = self.engine.thrsa_share_create(sec)
+        return self._shares[sec]
+
+    def sign_batch(self, secs: Sequence[bytes], reqs: Sequence[bytes]):
+        """[(serialized partial signature or None, error or None)], as Sign(sec, req) returns them."""
+        handles, idx, pos = [], [], {}
+        for s in secs:
+            h = self.register(s)
+            if h.value not in pos:
+                pos[h.value] = len(handles)
+                handles.append(h)
+            idx.append(pos[h.value])
+        err, outs = self.engine.thrsa_sign_batch(handles, idx, list(reqs))
+        res = []
+        for e, o in zip(err, outs):
+            if e == 0:
+                res.append((o if o else None, None))
+            else:
+                res.append((None, {-13: ErrInvalidInput, -8: "threshold rsa: malformed request"}.get(int(e), ErrNotBuilt)))
+        return res
+
+    def sign(self, sec: bytes, req: bytes):
+        return self.sign_batch([sec], [req])[0]
+
+    def process(self, n: int, k: int, responses: Sequence[bytes]):
+        """ProcessResponse over the responses so far (arrival order): (signature or None, error or None, index of the deciding
+        response or None, missing keys for the next MakeRequest)."""
+        state, err, at, sig, missing = self.engine.thrsa_process_batch(n, k, [list(responses)])[0]
+        if state == 1:
+            return sig, None, at, []
+        if state == 2:
+            return None, ({-8: "threshold rsa: malformed response"}.get(err, ErrNotBuilt)), at, []
+        return None, (None if missing else ErrInsufficientNumberOfThresholdSignatures), None, missing
+
+    def close(self):
+        for h in self._shares.values():
+            self.engine.thrsa_share_destroy(h)
+        self._shares = {}

@@ -14,6 +14,7 @@
 #include "pgp_parse.cuh"
 #include "msg_parse.cuh"
 #include "msg_decrypt.cuh"
+#include "thrsa_sign.cuh"
 #include "pgp_host.hpp"
 #include "wotqs_host.hpp"
 #include "bignum_host.hpp"
@@ -212,9 +213,12 @@ struct bftq_engine {
   uint32_t packer_flags = 0;   // BFTQ_F_* the packet-level entry points pass to K1 (bftq_engine_set_verify_flags / env BFTQ_STRICT_RANGE)
   std::mutex kr_mu;
   std::vector<bftq_keyring*> keyrings;           // live keyrings: their private-key tables are zeroed at shutdown
+  std::mutex thrsa_mu;
+  std::vector<bftq_thrsa_share*> thrsa_shares;   // live threshold-RSA shares: their fragments are zeroed at shutdown
 };
 void priv_release(bftq_keyring* kr);             // decrypt_host.inc: zero and free a keyring's private-key table
 void keyring_detach(bftq_keyring* kr);           // a keyring that outlives its engine becomes parse-only
+void thrsa_shutdown(bftq_engine* e);             // thrsa_host.inc: zero and free every live share's fragments
 
 namespace {
 
@@ -683,6 +687,7 @@ void bftq_shutdown(bftq_engine* e) {
     for (bftq_keyring* kr : e->keyrings) { priv_release(kr); keyring_detach(kr); }
     e->keyrings.clear();
   }
+  thrsa_shutdown(e);
   for (auto& kv : e->host_allocs) cudaFreeHost(kv.first);
   for (auto* s : e->slots) {
     if (s->stream) { cudaStreamSynchronize(s->stream); cudaStreamDestroy(s->stream); }
@@ -1745,6 +1750,7 @@ int bftq_pgp_digest_batch(bftq_engine* e, const uint8_t* data_blob, const uint64
 }  // extern "C"
 #include "packer_host.inc"
 #include "decrypt_host.inc"
+#include "thrsa_host.inc"
 
 // ---- quorum-descriptor builder ------------------------------------------------------------------
 // The descriptor the reference recomputes on EVERY call (client.go:64,101,141,238; server.go:182,211,237,300,473) is a

@@ -268,6 +268,64 @@ class Engine:
         _lib.check(self._lib.bftq_modprod_batch(self._h, _ptr(mb), mlen, k, _ptr(vb), B, _ptr(out)))
         return [bytes(o) for o in out]
 
+    # ---- K7: threshold-RSA partial signing and the client's combine (crypto/threshold/rsa/rsa.go) ----
+    def thrsa_share_create(self, sec: bytes):
+        """Registers one share (rsaContext's saved parameter) on the device; returns its handle."""
+        h = C.c_void_p()
+        buf = np.frombuffer(sec, np.uint8) if sec else np.zeros(1, np.uint8)
+        _lib.check(self._lib.bftq_thrsa_share_create(self._h, _ptr(buf), len(sec), C.byref(h)))
+        return h
+
+    def thrsa_share_destroy(self, share):
+        self._lib.bftq_thrsa_share_destroy(share)
+
+    @staticmethod
+    def _blob(items):
+        off = np.zeros(len(items) + 1, np.uint64)
+        off[1:] = np.cumsum([len(b) for b in items], dtype=np.uint64) if items else []
+        blob = np.frombuffer(b"".join(items), np.uint8) if off[-1] else np.zeros(1, np.uint8)
+        return blob, off
+
+    def thrsa_sign_batch(self, shares, share_idx, requests):
+        """rsaContext.Sign over (shares[share_idx[i]], requests[i]): (out_err int32[n], [serialized partial signatures])."""
+        n = len(requests)
+        blob, off = self._blob(list(requests))
+        tab = (C.c_void_p * max(1, len(shares)))(*[s.value for s in shares])
+        idx = np.ascontiguousarray(share_idx, np.uint32)
+        kids = [int.from_bytes(r[:2], "big") if len(r) >= 2 else 0 for r in requests]
+        cap = sum(2 + k * (12 + 256) + 8 + 256 for k in kids)
+        out = np.zeros(max(1, cap), np.uint8)
+        out_off = np.zeros(n + 1, np.uint64)
+        err = np.zeros(max(1, n), np.int32)
+        _lib.check(self._lib.bftq_thrsa_sign_batch(self._h, tab, len(shares), _ptr(idx), _ptr(blob), _ptr(off), n, _ptr(err),
+                                                   _ptr(out), cap, _ptr(out_off)))
+        return err[:n], [bytes(out[out_off[i]:out_off[i + 1]]) for i in range(n)]
+
+    def thrsa_process_batch(self, n: int, k: int, procs):
+        """rsaProc.ProcessResponse replayed over each process's responses (lists of bytes, arrival order).  Per process:
+        (state, err, at, signature bytes or None, missing key list)."""
+        P = len(procs)
+        flat = [r for rs in procs for r in rs]
+        blob, off = self._blob(flat)
+        poff = np.zeros(P + 1, np.uint64)
+        poff[1:] = np.cumsum([len(rs) for rs in procs], dtype=np.uint64) if procs else []
+        state, err = np.zeros(max(1, P), np.int32), np.zeros(max(1, P), np.int32)
+        at = np.zeros(max(1, P), np.uint64)
+        sig = np.zeros((max(1, P), 256), np.uint8)
+        moff = np.zeros(P + 1, np.uint64)
+        cap = 1 << 16
+        while True:
+            miss = np.zeros(cap, np.uint32)
+            rc = self._lib.bftq_thrsa_process_batch(self._h, n, k, _ptr(blob), _ptr(off), _ptr(poff), P, _ptr(state), _ptr(err), _ptr(at),
+                                                    _ptr(sig), _ptr(miss), cap, _ptr(moff))
+            if rc == -3 and moff[P] > cap:
+                cap = int(moff[P])
+                continue
+            _lib.check(rc)
+            break
+        return [(int(state[p]), int(err[p]), int(at[p]), bytes(sig[p]) if state[p] == 1 else None,
+                 [int(x) for x in miss[moff[p]:moff[p + 1]]]) for p in range(P)]
+
     def lagrange_exp_product_batch(self, p: int, q: int, x, ys):
         """auth.calculateSharedSecret: prod_j ys[i][j]^lambda_j mod p.  x: (B,k) ints, ys: B lists of k ints."""
         plen, qlen = (p.bit_length() + 7) // 8, (q.bit_length() + 7) // 8

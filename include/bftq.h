@@ -47,6 +47,7 @@ extern "C" {
 #define BFTQ_ERR_MESSAGE_BODY     -10   /* the literal body ends early / FileName is not base64: Decrypt returns that error as is */
 #define BFTQ_ERR_UNSUPPORTED      -11   /* a form the reference's library handles and this build does not (compressed data)       */
 #define BFTQ_ERR_MDC             -12   /* the SEIPD packet's modification detection code does not match: ReadAll's error, returned as is */
+#define BFTQ_ERR_INVALID_INPUT   -13   /* crypto.ErrInvalidInput (threshold RSA: the hash info leaves less than 3 padding bytes) */
 
 /* ---- per-item status bytes (SURVEY §8b "Errors") --------------------------------------------
  * The reference collapses every failure to ErrInvalidSignature (crypto_pgp.go:325-327); the shim
@@ -306,6 +307,50 @@ int bftq_modexp_batch(bftq_engine* e, const uint8_t* m_be, uint32_t mlen, const 
  * to len(N) like I2OS (rsa.go:380-393).  N: exactly 1024 or 2048 bits; vals: n_items x k x mlen. */
 int bftq_modprod_batch(bftq_engine* e, const uint8_t* m_be, uint32_t mlen, uint32_t k, const uint8_t* vals_be, uint64_t n_items,
                        uint8_t* out_be);
+/* ---- K7: threshold-RSA partial signing (crypto/threshold/rsa/rsa.go) ----------------------------
+ * A share is rsaContext's saved parameter: the bytes of ThresholdInstance's secret after its algo byte (TH_RSA only),
+ * serializePartialParam's framing (rsa.go:409-485): u16 count, per fragment u32 key index, a sign byte and a u64-length
+ * chunk (big-endian magnitude; an empty chunk is the fragment 0), then the N chunk, u32 id, u8 n.  Registration is opt-in:
+ * the fragments go to one device allocation per share, zeroed before it is freed (bftq_thrsa_share_destroy,
+ * bftq_shutdown); the host copies are wiped after upload and no key material reaches stats or error texts.
+ *   BFTQ_ERR_MALFORMED        framing error (truncated share)
+ *   BFTQ_ERR_UNSUPPORTED_KEY  N not odd with exactly 2048 bits, or a fragment longer than 8192 bytes (splitKey's depth
+ *                             n - k <= 4): the shim keeps such a share on the Go path */
+typedef struct bftq_thrsa_share bftq_thrsa_share;
+int bftq_thrsa_share_create(bftq_engine* e, const uint8_t* sec, uint64_t len, bftq_thrsa_share** out);
+void bftq_thrsa_share_destroy(bftq_thrsa_share* s);
+/* rsaContext.Sign (rsa.go:140-178) over n_items (share, serialized sign request) pairs: item i signs request
+ * req_blob[req_off[i] .. req_off[i+1]) with shares[share_idx[i]] (share_idx[i] < n_shares).  Output: item i's
+ * serializePartialSignature bytes at out_blob[out_off[i] .. out_off[i+1]), packed; u16 count, per distinct index
+ * kid * n + id + 1 (uint32 arithmetic) a u32 index and the chunk of the partial signature's minimal big-endian bytes,
+ * then the N chunk.  Go writes the entries in map order (random); here they follow the order in which the request
+ * first lists their index.  A request listing the same key id twice with a negative fragment yields m^|d| for it, as
+ * the reference's in-place Neg does.  out_cap must hold the sum over items of  2 + kids (12 + 256) + 8 + 256  bytes
+ * (kids: the request's key-id count), else BFTQ_ERR_INVALID_ARG before any work.
+ *   out_err[i]  0 (an item whose request names no key id of the share: length 0, Sign's (nil, nil)) |
+ *               BFTQ_ERR_MALFORMED (request framing) | BFTQ_ERR_INVALID_INPUT (emsaEncode's padlen < 3) |
+ *               BFTQ_ERR_UNSUPPORTED (m is not invertible mod N: only with a factor of N) */
+int bftq_thrsa_sign_batch(bftq_engine* e, bftq_thrsa_share* const* shares, uint32_t n_shares, const uint32_t* share_idx,
+                          const uint8_t* req_blob, const uint64_t* req_off, uint64_t n_items, int32_t* out_err, uint8_t* out_blob,
+                          uint64_t out_cap, uint64_t* out_off);
+/* rsaProc.ProcessResponse (rsa.go:235-338) replayed, statelessly, over each process's responses in arrival order:
+ * process p's responses are r = proc_off[p] .. proc_off[p+1]), response r at resp_blob[resp_off[r] .. resp_off[r+1]).
+ * n (>= 2) and k are the Threshold's.  Processing stops at the first response that yields a signature or an error, as
+ * the DistSign callback does; out_at[p] is its index within the process (the response count when none did).  The
+ * first partial signature registered at an index wins; a response's entries register in the order it lists them (Go:
+ * map order); N is the completing response's.  Completed products run on the device (K5 modprod, one launch per N).
+ *   out_state[p]  BFTQ_THRSA_SIGNED: out_sig[p * 256 ..] = I2OS(s, 256) | BFTQ_THRSA_FAILED: out_err[p] = BFTQ_ERR_MALFORMED
+ *                 (a response does not parse) or BFTQ_ERR_UNSUPPORTED_KEY (the completing N is not odd 2048-bit, or a
+ *                 partial signature exceeds 512 bytes: the shim combines on big.Int) | BFTQ_THRSA_INCOMPLETE: the
+ *                 missingKeys list for the next MakeRequest at out_missing[out_missing_off[p] .. out_missing_off[p+1])
+ *                 (empty: MakeRequest returns no request, ErrInsufficientNumberOfThresholdSignatures).
+ * missing_cap: capacity of out_missing in entries (BFTQ_ERR_INVALID_ARG when the lists do not fit). */
+#define BFTQ_THRSA_INCOMPLETE 0
+#define BFTQ_THRSA_SIGNED     1
+#define BFTQ_THRSA_FAILED     2
+int bftq_thrsa_process_batch(bftq_engine* e, uint32_t n, uint32_t k, const uint8_t* resp_blob, const uint64_t* resp_off,
+                             const uint64_t* proc_off, uint64_t n_procs, int32_t* out_state, int32_t* out_err, uint64_t* out_at,
+                             uint8_t* out_sig, uint32_t* out_missing, uint64_t missing_cap, uint64_t* out_missing_off);
 /* AuthClient.calculateSharedSecret (crypto/auth/auth.go:386-399) and the first half of CalculateR:
  * out[i] = prod_j y[i][j]^lambda_j mod p,  lambda_j = sss.Lagrange(x[i][j], x[i][*], q).
  * p: plen = 128/256 bytes; q: any odd modulus up to 256 bytes (auth uses q = (p-1)/2). */
