@@ -3,13 +3,14 @@
 // public_key.go: digest cut to the subgroup size) and Go crypto/dsa.Verify:
 //     0 < r, s < q;  w = s^-1 mod q;  u1 = z w, u2 = r w mod q;  v = (g^u1 y^u2 mod p) mod q;  valid iff v == r
 // Three stages per key (p, q, g, y):
-//   dsa_prepare_kernel   thread per signature: range checks, w by Fermat (q prime), u1 / u2         (this file)
+//   dsa_prepare_kernel   thread per signature: range checks, w = s^-1 mod q, u1 / u2                 (this file)
 //   modexp_kernel        2 items per signature: g^u1, y^u2 (bases broadcast)  +  modprod_kernel      (modexp.cuh)
 //   dsa_finish_kernel    thread per signature: (product mod q) == r                                  (this file)
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
 #include "lagrange.cuh"
+#include "modinv_big.cuh"
 
 namespace bftq {
 
@@ -65,6 +66,22 @@ dsa_prepare_kernel(const LagrangeMod<L> M, const uint8_t* __restrict__ r_be, con
   for (int bit = 32 * L - 1; bit >= 0; bit--) {
     mont_mul_big<L>(acc, acc, acc, M);
     if ((e[bit >> 5] >> (bit & 31)) & 1u) mont_mul_big<L>(acc, acc, sm, M);
+  }
+  // acc = s^(q-2) R is s^-1 R only when q is prime, and q is the key holder's choice (nothing checks that it is prime).
+  // (w R) s / R == 1 proves w exact (the inverse is unique); otherwise w comes from the extended GCD, and when
+  // gcd(s, q) != 1 there is none: dsa.Verify's ModInverse returns nil and the signature is false.
+  mont_mul_big<L>(t, acc, s, M);
+  bool one = t[0] == 1u;
+#pragma unroll
+  for (int l = 1; l < L; l++) one = one && t[l] == 0u;
+  if (!one) {
+    uint32_t w[L];
+    if (!modinv_big<L>(w, s, M.m)) {
+      for (int b = 0; b < 2 * mlen; b++) up[b] = 0;
+      status[item] = 1;
+      return;
+    }
+    mont_mul_big<L>(acc, w, M.r2, M);                                 // w R
   }
   mont_mul_big<L>(t, z, acc, M);                                      // z (w R) / R = z w
   store_be_right<L>(up, mlen, t);
