@@ -169,6 +169,7 @@ struct EdCache {
   uint64_t resets = 0;                           // times a full cache was emptied for a batch that pays for its tables
   std::map<std::string, uint32_t> slot_of;       // 32 key bytes -> slot
   std::vector<cudaEvent_t> pending;              // builds that may still be running
+  bool enabled = true;                           // BFTQ_ED25519_TABLES, read when the engine is created
 };
 
 // Large device scratch blocks kept across calls (bftq_read_responses_batch needs about 2.5 x the raw answers; a
@@ -640,6 +641,7 @@ int bftq_init(int device, bftq_engine** out) {
   e->device = device;
   e->sm_count = prop.multiProcessorCount;
   if (env_on("BFTQ_STRICT_RANGE", false)) e->packer_flags |= BFTQ_F_STRICT_RANGE;
+  e->ed.enabled = env_on("BFTQ_ED25519_TABLES", true);
   numa_probe(e);
   e->pool.on_start = [e] { numa_bind_this_thread(e); };
   *out = e;
@@ -1002,8 +1004,7 @@ int bftq_ed25519_verify_batch_dev(bftq_engine* e, const uint8_t* pubkeys, uint32
   // about 1 000 such verifications' worth of work once per key and engine (about 100 table-free ones), so a batch may
   // bring one NEW key per 32 signatures; keys that are cached already cost nothing, whatever the batch size.  Batches
   // with more new keys than that (every signature under its own key, say) take the table-free double-and-add kernel.
-  static const bool no_tables = !env_on("BFTQ_ED25519_TABLES", true);
-  bool tables = !no_tables && n_keys > 0 && n_keys <= 4096;
+  bool tables = e->ed.enabled && n_keys > 0 && n_keys <= 4096;
   int launches = 0;
   if (tables) {
     std::vector<uint32_t> slot_of_key;

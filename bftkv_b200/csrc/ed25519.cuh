@@ -4,10 +4,14 @@
 // library (golang.org/x/crypto/openpgp @53104e6ec876) has no EdDSA (public-key algorithm 22) and
 // skips such keys (SURVEY F5), so there is no reference behaviour to be bit-identical with.  The
 // semantics here are RFC 8032 §5.1.7 as Go's crypto/ed25519 / ref10 / OpenSSL implement it:
-//   reject S >= L;  decode A (reject y >= p, reject non-square, reject x = 0 with sign bit set);
-//   k = SHA-512(R || A || M) mod L;  accept iff  encode([S]B - [k]A) == R  (byte compare).
+//   reject S >= L;  decode A as edwards25519.Point.SetBytes does: y = the low 255 bits reduced mod p (y >= p is
+//   accepted), reject only when (y^2 - 1) / (d y^2 + 1) is not a square, x = 0 with the sign bit set is accepted;
+//   k = SHA-512(R || A || M) mod L over the caller's raw 32 key bytes;  accept iff  encode([S]B - [k]A) == R (byte
+//   compare: R is never decoded, so a non-canonical R never matches).  No cofactor: small-order and mixed-order A and R
+//   are decided by this equation alone.  libsodium is stricter (it rejects small-order A and R and non-canonical A).
 // In OpenPGP (RFC 4880bis / GnuPG) M is the 32-byte v4 signature digest, so messages are a fixed 32
-// bytes here.  Parity oracle for this kernel: libsodium (pynacl) and OpenSSL (`cryptography`).
+// bytes here.  Parity oracle for this kernel: a restatement of Go's Verify (oracle/ed25519_oracle.py) and OpenSSL
+// (`cryptography`); libsodium (pynacl) wherever it is not stricter.
 //
 // This file: the table-free kernel (batches with few signatures per key) and the shared field / group / scalar code;
 // ed25519_fast.cuh holds the cached-window-table path every large batch takes.
@@ -136,7 +140,8 @@ BFTQ_HD_NOINLINE void fe_tobytes(uint8_t* s, const fe hin) {
   if (wi < 8) w[wi++] = (uint32_t)acc;
   for (int i = 0; i < 8; i++) { s[4 * i] = (uint8_t)w[i]; s[4 * i + 1] = (uint8_t)(w[i] >> 8); s[4 * i + 2] = (uint8_t)(w[i] >> 16); s[4 * i + 3] = (uint8_t)(w[i] >> 24); }
 }
-// Loads 255 bits (the top bit is ignored).  Returns false when the value is >= p (non-canonical).
+// Loads 255 bits (the top bit is ignored); values in [p, 2^255) stay as they are, a valid representative of value - p.
+// Returns false when the value is >= p (non-canonical).
 BFTQ_HD bool fe_frombytes(fe h, const uint8_t* s) {
   uint32_t w[8];
   for (int i = 0; i < 8; i++) w[i] = (uint32_t)s[4 * i] | ((uint32_t)s[4 * i + 1] << 8) | ((uint32_t)s[4 * i + 2] << 16) | ((uint32_t)s[4 * i + 3] << 24);
@@ -238,10 +243,11 @@ BFTQ_HD_NOINLINE void ge_dbl(ge& r, const ge& p) {
   // f = c + g can reach 2^27 per limb: keep it the FIRST operand (the second one is pre-multiplied by 19 in 32 bits)
   fe_mul(r.X, f, e); fe_mul(r.Y, g, h); fe_mul(r.T, e, h); fe_mul(r.Z, f, g);
 }
-// RFC 8032 §5.1.3 decoding.  false = not a curve point / non-canonical.
+// Point decoding as Go's edwards25519.Point.SetBytes and OpenSSL do it: RFC 8032 §5.1.3 except that y >= p is taken mod p
+// and x = 0 with the sign bit set is accepted (x stays 0).  false = (y^2 - 1) / (d y^2 + 1) has no square root.
 BFTQ_HD bool ge_frombytes(ge& p, const uint8_t* s) {
   const int sign = s[31] >> 7;
-  if (!fe_frombytes(p.Y, s)) return false;
+  fe_frombytes(p.Y, s);                    // y >= p: the limbs hold y, which is y - p mod p
   fe u, v, v3, x, vxx, chk;
   fe_1(p.Z);
   fe_sq(u, p.Y);
@@ -259,8 +265,7 @@ BFTQ_HD bool ge_frombytes(ge& p, const uint8_t* s) {
     if (!fe_iszero(chk)) return false;
     fe_mul(x, x, BFTQ_ED_TAB(kSqrtM1));
   }
-  if (fe_iszero(x) && sign) return false;
-  if ((int)fe_isnegative(x) != sign) fe_neg(x, x);
+  if ((int)fe_isnegative(x) != sign) fe_neg(x, x);   // x = 0: -0 = 0
   fe_copy(p.X, x);
   fe_mul(p.T, p.X, p.Y);
   return true;

@@ -13,8 +13,9 @@
 //     simultaneous inversion over eight results per thread;
 //   * k = SHA-512(R || A || M) mod L is a Barrett reduction (81 + 45 word products) instead of 512 shift-subtract steps.
 // Per verification: ~47.9 * 7 = 335 field products in kernel 1 + ~25 in kernel 2 (about 36 000 32x32->64 multiplies)
-// instead of ~1 230 (135 000).  Semantics are unchanged (RFC 8032 §5.1.7 as Go's crypto/ed25519 / OpenSSL implement it:
-// S < L, canonical decodable A, byte compare of the encoding of [S]B - [k]A with R).
+// instead of ~1 230 (135 000).  Semantics are those of ed25519.cuh (RFC 8032 §5.1.7 as Go's crypto/ed25519 / OpenSSL
+// implement it: S < L; A decoded as edwards25519.Point.SetBytes does, y reduced mod p and x = 0 with the sign bit allowed;
+// k over the raw key bytes; byte compare of the encoding of [S]B - [k]A with R; no cofactor).
 // Everything is __host__ __device__: tests/harness/ed25519_host.cpp runs the same code on the CPU against OpenSSL,
 // libsodium and the RFC 8032 vectors.
 #pragma once
@@ -243,10 +244,11 @@ BFTQ_HDI void gex_identity(gex& p) {
 BFTQ_HD void gex_basepoint(gex& b) {
   for (int i = 0; i < 10; i++) { b.X[i] = BFTQ_ED_TAB(kBx)[i]; b.Y[i] = BFTQ_ED_TAB(kBy)[i]; b.Z[i] = (i == 0); b.T[i] = BFTQ_ED_TAB(kBt)[i]; }
 }
-// RFC 8032 §5.1.3 decoding with the inlined field (same decisions as ge_frombytes).
+// Point decoding with the inlined field, the same decisions as ge_frombytes: y >= p is taken mod p, x = 0 with the sign bit
+// set is accepted; false only when x^2 has no square root.  Two encodings of one point are two cache slots.
 BFTQ_HD_NOINLINE bool gex_frombytes(gex& p, const uint8_t* s) {
   const int sign = s[31] >> 7;
-  if (!fe_frombytes(p.Y, s)) return false;
+  fe_frombytes(p.Y, s);                    // y >= p: the limbs hold y, which is y - p mod p
   int32_t u[10], v[10], v3[10], x[10], t[10], vxx[10], chk[10], one[10], kd[10], ksm1[10];
   for (int i = 0; i < 10; i++) { one[i] = (i == 0); kd[i] = BFTQ_ED_TAB(kD)[i]; ksm1[i] = BFTQ_ED_TAB(kSqrtM1)[i]; }
   fex_copy(p.Z, one);
@@ -265,8 +267,7 @@ BFTQ_HD_NOINLINE bool gex_frombytes(gex& p, const uint8_t* s) {
     if (!fe_iszero(chk)) return false;
     fex_mul(t, x, ksm1); fex_copy(x, t);
   }
-  if (fe_iszero(x) && sign) return false;
-  if ((int)fe_isnegative(x) != sign) { for (int i = 0; i < 10; i++) x[i] = -x[i]; }
+  if ((int)fe_isnegative(x) != sign) { for (int i = 0; i < 10; i++) x[i] = -x[i]; }   // x = 0: -0 = 0
   fex_copy(p.X, x);
   fex_mul(p.T, p.X, p.Y);
   return true;

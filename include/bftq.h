@@ -162,7 +162,10 @@ int bftq_rsa_verify_batch_dev_k(bftq_engine* e, uint32_t key_bytes, const uint32
  * EdDSA (algorithm 22) and skips such keys.  RFC 8032 pure Ed25519 as GnuPG uses it in OpenPGP: the
  * signed "message" is the 32-byte v4 signature digest.  pubkeys: n_keys x 32 (compressed A),
  * sig: n_items x 64 (R || S), msg: n_items x 32.  out_status: BFTQ_ST_OK / _BAD_SIGNATURE /
- * _UNKNOWN_SIGNER.  Rejects S >= L and non-canonical / off-curve A like Go's crypto/ed25519.
+ * _UNKNOWN_SIGNER.  Decides as Go's crypto/ed25519 (1.17 and later) and OpenSSL do: rejects S >= L; decodes A as
+ * edwards25519.Point.SetBytes does (y >= p is reduced mod p, x = 0 with the sign bit set is accepted, an A with no
+ * square root is rejected); hashes the raw 32 key bytes; compares the encoding of [S]B - [k]A with R's bytes; no
+ * cofactor.  libsodium is stricter: it also rejects small-order A and R and non-canonical A.
  * Keys are metadata, like the RSA key table: `pubkeys` is HOST memory in both forms (the _dev form takes the bulk arrays
  * key_idx / sig / msg / status in device memory).  Batches run against window tables that the engine caches: one for
  * the base point (5.8 MB) and one per key (1.7 MB each, built on first sight of the 32 key bytes, bounded by

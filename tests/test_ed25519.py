@@ -30,8 +30,8 @@ RFC8032 = [
 def host():
     so = os.path.join(ROOT, "tests", "harness", "libedhost.so")
     src = os.path.join(ROOT, "tests", "harness", "ed25519_host.cpp")
-    hdr = os.path.join(ROOT, "bftkv_b200", "csrc", "ed25519.cuh")
-    if not os.path.exists(so) or os.path.getmtime(so) < max(os.path.getmtime(src), os.path.getmtime(hdr)):
+    hdrs = [os.path.join(ROOT, "bftkv_b200", "csrc", h) for h in ("ed25519.cuh", "ed25519_fast.cuh")]
+    if not os.path.exists(so) or os.path.getmtime(so) < max(os.path.getmtime(f) for f in [src] + hdrs):
         subprocess.check_call(["g++", "-O2", "-shared", "-fPIC", "-o", so, src])
     return ctypes.CDLL(so)
 
@@ -106,7 +106,7 @@ def test_rfc8032_vectors_and_openssl(host):
         except nacl.exceptions.BadSignatureError:
             sodium = False
         assert got == sodium
-    # non-canonical S (S + L), non-canonical / off-curve A
+    # non-canonical S (S + L); keys the signature is not for: y = p + 1 (the identity), y = 2 (no point), ff..ff (y = p + 18)
     s0 = sig[0].tobytes()
     S = int.from_bytes(s0[32:], "little") + L
     pk0, m0 = pks[kidx[0]], msg[0].tobytes()

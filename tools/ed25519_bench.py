@@ -1,5 +1,5 @@
 """K1b on one GPU: 262 144 Ed25519 verifies over 15 keys (BASELINE configs[3]), device-resident, CUDA events.
-BFTQ_ED25519_TABLES=0 selects the classic double-and-add kernel (one process per setting: the switch is read once)."""
+BFTQ_ED25519_TABLES=0 selects the classic double-and-add kernel (the switch is read when the engine is created)."""
 import os
 import sys
 import time
