@@ -741,28 +741,20 @@ int make_key_consts(const uint8_t* n_be, uint32_t stride, uint32_t exp, bftq::Rs
   if (exp == 0) return fail(BFTQ_ERR_UNSUPPORTED_KEY, "public exponent 0");
   memset(&kd, 0, sizeof(kd));
   to_digits(n, kd.n, bftq::kMaxDigits);
-  // -n^-1 mod 2^32 by Newton iteration on the low word (masked to 28 bits for the digit kernels).
-  uint32_t n0 = (uint32_t)n.w[0], inv = n0;
-  for (int i = 0; i < 5; i++) inv *= 2u - n0 * inv;
-  kd.n0inv = (0u - inv) & bftq::kDigitMask;
+  const uint32_t n0inv = neg_inv32((uint32_t)n.w[0]);
+  kd.n0inv = n0inv & bftq::kDigitMask;                   // -n^-1 mod 2^28 for the digit kernels
   kd.e = exp;
   kd.nbits = (uint32_t)nb;
   kd.kbytes = (uint32_t)kb;
-  // R^2 mod n for each digit layout of the class: 2^(2*28*digits) by repeated doubling from 1.
-  UBig x;
-  memset(&x, 0, sizeof(x));
-  x.w[0] = 1;
-  int exp2 = 0;
-  for (int layout = 0; layout < bftq::kNumLayouts; layout++) {
-    const int digits = bftq::class_digits(cls, layout == 1 && cls != 256 ? 0 : layout);
-    const int target = 2 * 28 * digits;
-    while (exp2 < target) { dbl_mod(x, n); exp2++; }
-    if (exp2 == target) to_digits(x, kd.r2[layout], bftq::kMaxDigits);
-  }
+  // R^2 mod n for the class's digit layout: 2^(2*28*digits) by repeated doubling from 1.
+  UBig one;
+  memset(&one, 0, sizeof(one));
+  one.w[0] = 1;
+  to_digits(shl_mod(one, n, 2 * 28 * bftq::class_digits(cls)), kd.r2, bftq::kMaxDigits);
   // radix-2^32 constants (fast path, meaningful for exactly-2048-bit moduli): n, -n^-1 mod 2^32, the verification constants
   memset(&k32, 0, sizeof(k32));
   to_words(n, k32.n, 64);
-  k32.n0inv = 0u - inv;
+  k32.n0inv = n0inv;
   k32.e = exp;
   k32.nbits = (uint32_t)nb;
   if (nb == 2048) {
@@ -1340,9 +1332,7 @@ void make_lagrange_mod(const uint8_t* m_be, uint32_t mlen, bftq::LagrangeMod<L>&
     M.m[bi >> 2] |= (uint32_t)m_be[i] << (8 * (bi & 3));
   }
   M.mlen = mlen;
-  uint32_t inv = M.m[0];
-  for (int i = 0; i < 5; i++) inv *= 2u - M.m[0] * inv;
-  M.m0inv = 0u - inv;
+  M.m0inv = neg_inv32(M.m[0]);
   // R mod m and R^2 mod m by shift-and-subtract from 1
   std::vector<uint32_t> r(L + 1, 0u);
   r[0] = 1;
@@ -1404,16 +1394,13 @@ int make_moddev(const uint8_t* p_be, uint32_t plen, bftq::ModDev<W>& M) {
   from_be(n, p_be, plen);
   if (bitlen(n) != 128 * W || !(n.w[0] & 1)) return fail(BFTQ_ERR_UNSUPPORTED_KEY, "exponentiation modulus must be odd with exactly 8*len bits");
   memset(&M, 0, sizeof(M));
-  for (int i = 0; i < 2 * W; i++) { M.n[2 * i] = (uint32_t)n.w[i]; M.n[2 * i + 1] = (uint32_t)(n.w[i] >> 32); }
-  uint32_t n0 = (uint32_t)n.w[0], inv = n0;
-  for (int i = 0; i < 5; i++) inv *= 2u - n0 * inv;
-  M.n0inv = 0u - inv;
+  to_words(n, M.n, 4 * W);
+  M.n0inv = neg_inv32(M.n[0]);
   M.nbytes = plen;
-  UBig y;
-  memset(&y, 0, sizeof(y));
-  y.w[0] = 1;
-  for (int ex = 0; ex < 2 * 128 * W; ex++) dbl_mod(y, n);
-  for (int i = 0; i < 2 * W; i++) { M.r2[2 * i] = (uint32_t)y.w[i]; M.r2[2 * i + 1] = (uint32_t)(y.w[i] >> 32); }
+  UBig one;
+  memset(&one, 0, sizeof(one));
+  one.w[0] = 1;
+  to_words(shl_mod(one, n, 2 * 128 * W), M.r2, 4 * W);
   return BFTQ_OK;
 }
 template <int W>

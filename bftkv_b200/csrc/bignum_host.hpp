@@ -50,6 +50,19 @@ inline void to_words(const UBig& a, uint32_t* w, int nw) {
   for (int i = 0; i < nw; i++) w[i] = (uint32_t)(a.w[i / 2] >> (32 * (i & 1)));
 }
 
+// -n^-1 mod 2^32 / 2^64 for odd n (Montgomery's n0inv), by Newton iteration: each step doubles the correct low bits
+// (3 -> 96).
+inline uint32_t neg_inv32(const uint32_t n0) {
+  uint32_t inv = n0;
+  for (int i = 0; i < 5; i++) inv *= 2u - n0 * inv;
+  return 0u - inv;
+}
+inline uint64_t neg_inv64(const uint64_t n0) {
+  uint64_t inv = n0;
+  for (int i = 0; i < 5; i++) inv *= 2u - n0 * inv;
+  return 0u - inv;
+}
+
 // a * b * 2^-2048 mod n for a, b < n, n odd and below 2^2048; n0inv = -n^-1 mod 2^64.  Word-serial Montgomery product.
 inline UBig mont2048(const UBig& a, const UBig& b, const UBig& n, const uint64_t n0inv) {
   constexpr int L = 32;
@@ -90,9 +103,7 @@ inline UBig mont2048(const UBig& a, const UBig& b, const UBig& n, const uint64_t
 //   c16 = c * 2^512,  hc16 = (2^2033 - 2^512) * c,  c32 = c * 2^1024,  hc32 = (2^2033 - 2^1024) * c   (all mod n)
 struct VerifyConsts { UBig c16, hc16, c32, hc32; };
 inline VerifyConsts verify_consts(const UBig& n, const uint32_t e) {
-  uint64_t inv = n.w[0];                                  // n^-1 mod 2^64 by Newton iteration (3 -> 96 bits)
-  for (int i = 0; i < 5; i++) inv *= 2u - n.w[0] * inv;
-  const uint64_t n0inv = 0u - inv;
+  const uint64_t n0inv = neg_inv64(n.w[0]);
   UBig one;
   memset(&one, 0, sizeof(one));
   one.w[0] = 1;

@@ -10,23 +10,10 @@
 #include <cstdint>
 #include <cuda_runtime.h>
 #include "lagrange.cuh"
+#include "limbs.cuh"
 #include "modinv_big.cuh"
 
 namespace bftq {
-
-template <int L>
-__device__ __forceinline__ void load_be_right(uint32_t (&v)[L], const uint8_t* p, int nbytes) {
-#pragma unroll
-  for (int l = 0; l < L; l++) {
-    uint32_t w = 0;
-    for (int b = 0; b < 4; b++) { const int pos = nbytes - 1 - (4 * l + b); if (pos >= 0) w |= (uint32_t)__ldg(p + pos) << (8 * b); }
-    v[l] = w;
-  }
-}
-template <int L>
-__device__ __forceinline__ void store_be_right(uint8_t* p, int nbytes, const uint32_t (&v)[L]) {
-  for (int q = 0; q < nbytes; q++) { const int bi = nbytes - 1 - q; p[q] = (uint8_t)(v[bi >> 2] >> (8 * (bi & 3))); }
-}
 
 // r_be / s_be: 32-byte right-aligned values `stride` bytes apart, digest: n x dlen.  u_be: 2n x mlen (u1, u2 interleaved).
 // status: BFTQ_ST_OK to continue, 1 when dsa.Verify already says false; a non-zero pre[] entry is copied.
@@ -39,34 +26,23 @@ dsa_prepare_kernel(const LagrangeMod<L> M, const uint8_t* __restrict__ r_be, con
   if (item >= n_items) return;
   const int mlen = (int)M.mlen;
   uint8_t* up = u_be + 2 * item * (uint64_t)mlen;
-  uint32_t r[L], s[L], z[L], e[L], acc[L], sm[L], t[L];
-  load_be_right<L>(r, r_be + item * stride, 32);
-  load_be_right<L>(s, s_be + item * stride, 32);
+  uint32_t r[L], s[L], z[L], acc[L], t[L];
+  limbs::load_be<L>(r, r_be + item * stride, 32);
+  limbs::load_be<L>(s, s_be + item * stride, 32);
   bool rz = true, sz = true;
 #pragma unroll
   for (int l = 0; l < L; l++) { rz = rz && r[l] == 0; sz = sz && s[l] == 0; }
   uint8_t st = (pre != nullptr) ? pre[item] : 0;
-  if (!st && (rz || sz || ge_big<L>(r, M.m) || ge_big<L>(s, M.m))) st = 1;
+  if (!st && (rz || sz || limbs::ge<L>(r, M.m) || limbs::ge<L>(s, M.m))) st = 1;
   if (st) {
     for (int b = 0; b < 2 * mlen; b++) up[b] = 0;
     status[item] = st;
     return;
   }
   const int take = (int)dlen < mlen ? (int)dlen : mlen;                 // hashBytes[:subgroupSize]
-  load_be_right<L>(z, digest + item * (uint64_t)dlen, take);
-  if (ge_big<L>(z, M.m)) sub_big<L>(z, M.m);                          // z < 2^(8 mlen) < 2q (q has exactly 8 mlen bits)
-#pragma unroll
-  for (int l = 0; l < L; l++) e[l] = M.m[l];
-  uint32_t br = 2;
-#pragma unroll
-  for (int l = 0; l < L; l++) { const uint64_t d = (uint64_t)e[l] - br; e[l] = (uint32_t)d; br = (uint32_t)(d >> 63); }
-  mont_mul_big<L>(sm, s, M.r2, M);
-#pragma unroll
-  for (int l = 0; l < L; l++) acc[l] = M.r1[l];
-  for (int bit = 32 * L - 1; bit >= 0; bit--) {
-    mont_mul_big<L>(acc, acc, acc, M);
-    if ((e[bit >> 5] >> (bit & 31)) & 1u) mont_mul_big<L>(acc, acc, sm, M);
-  }
+  limbs::load_be<L>(z, digest + item * (uint64_t)dlen, take);
+  if (limbs::ge<L>(z, M.m)) limbs::sub<L>(z, M.m);                          // z < 2^(8 mlen) < 2q (q has exactly 8 mlen bits)
+  fermat_pow<L>(acc, s, M);
   // acc = s^(q-2) R is s^-1 R only when q is prime, and q is the key holder's choice (nothing checks that it is prime).
   // (w R) s / R == 1 proves w exact (the inverse is unique); otherwise w comes from the extended GCD, and when
   // gcd(s, q) != 1 there is none: dsa.Verify's ModInverse returns nil and the signature is false.
@@ -84,9 +60,9 @@ dsa_prepare_kernel(const LagrangeMod<L> M, const uint8_t* __restrict__ r_be, con
     mont_mul_big<L>(acc, w, M.r2, M);                                 // w R
   }
   mont_mul_big<L>(t, z, acc, M);                                      // z (w R) / R = z w
-  store_be_right<L>(up, mlen, t);
+  limbs::store_be_bytes<L>(up, mlen, t);
   mont_mul_big<L>(t, r, acc, M);
-  store_be_right<L>(up + mlen, mlen, t);
+  limbs::store_be_bytes<L>(up + mlen, mlen, t);
   status[item] = 0;
 }
 
@@ -99,25 +75,9 @@ dsa_finish_kernel(const LagrangeMod<L> M, const uint8_t* __restrict__ prod_be, c
   const uint64_t item = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (item >= n_items) return;
   if (status[item] != 0) return;
-  uint32_t v[L + 1], r[L];
-#pragma unroll
-  for (int l = 0; l <= L; l++) v[l] = 0;
-  const uint8_t* bp = prod_be + item * (uint64_t)nbytes;
-  for (uint32_t by = 0; by < nbytes; by++) {
-    const uint32_t byte = __ldg(bp + by);
-    for (int bit = 7; bit >= 0; bit--) {
-      uint32_t c = (byte >> bit) & 1u;
-#pragma unroll
-      for (int l = 0; l <= L; l++) { const uint32_t nc = v[l] >> 31; v[l] = (v[l] << 1) | c; c = nc; }
-      if (v[L] != 0 || ge_big<L>(v, M.m)) {
-        uint32_t br = 0;
-#pragma unroll
-        for (int l = 0; l < L; l++) { const uint64_t d = (uint64_t)v[l] - M.m[l] - br; v[l] = (uint32_t)d; br = (uint32_t)(d >> 63); }
-        v[L] -= br;
-      }
-    }
-  }
-  load_be_right<L>(r, r_be + item * stride, 32);
+  uint32_t v[L], r[L];
+  limbs::reduce_be<L>(v, prod_be + item * (uint64_t)nbytes, nbytes, M.m);
+  limbs::load_be<L>(r, r_be + item * stride, 32);
   bool eq = true;
 #pragma unroll
   for (int l = 0; l < L; l++) eq = eq && v[l] == r[l];

@@ -17,6 +17,7 @@
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
+#include "limbs.cuh"
 
 namespace bftq {
 
@@ -29,24 +30,6 @@ struct LagrangeMod {
   uint32_t mlen;        // bytes of m (output width)
 };
 
-template <int L>
-__device__ __forceinline__ bool ge_big(const uint32_t* a, const uint32_t* b) {
-#pragma unroll
-  for (int i = L - 1; i >= 0; i--) {
-    if (a[i] != b[i]) return a[i] > b[i];
-  }
-  return true;
-}
-template <int L>
-__device__ __forceinline__ void sub_big(uint32_t* a, const uint32_t* b) {
-  uint32_t br = 0;
-#pragma unroll
-  for (int i = 0; i < L; i++) {
-    const uint64_t d = (uint64_t)a[i] - b[i] - br;
-    a[i] = (uint32_t)d;
-    br = (uint32_t)(d >> 63);
-  }
-}
 // r = a*b*R^-1 mod m, fully reduced.  a < m; b < R.
 template <int L>
 __device__ void mont_mul_big(uint32_t* r, const uint32_t* a, const uint32_t* b, const LagrangeMod<L>& M) {
@@ -79,9 +62,27 @@ __device__ void mont_mul_big(uint32_t* r, const uint32_t* a, const uint32_t* b, 
     t[L - 1] = (uint32_t)v;
     t[L] = t[L + 1] + (uint32_t)(v >> 32);
   }
-  if (t[L] != 0 || ge_big<L>(t, M.m)) sub_big<L>(t, M.m);
+  if (t[L] != 0 || limbs::ge<L>(t, M.m)) limbs::sub<L>(t, M.m);
 #pragma unroll
   for (int i = 0; i < L; i++) r[i] = t[i];
+}
+
+// acc = v^(m-2) R mod m (Montgomery form; v^-1 R when m is prime), v < m plain.  Square-and-multiply over all 32 L bits.
+template <int L>
+__device__ __forceinline__ void fermat_pow(uint32_t (&acc)[L], const uint32_t (&v)[L], const LagrangeMod<L>& M) {
+  uint32_t e[L], vm[L];
+#pragma unroll
+  for (int l = 0; l < L; l++) e[l] = M.m[l];
+  uint32_t br = 2;                                                  // e = m - 2
+#pragma unroll
+  for (int l = 0; l < L; l++) { const uint64_t d = (uint64_t)e[l] - br; e[l] = (uint32_t)d; br = (uint32_t)(d >> 63); }
+  mont_mul_big<L>(vm, v, M.r2, M);                                  // v R
+#pragma unroll
+  for (int l = 0; l < L; l++) acc[l] = M.r1[l];                     // 1 R
+  for (int bit = 32 * L - 1; bit >= 0; bit--) {
+    mont_mul_big<L>(acc, acc, acc, M);
+    if ((e[bit >> 5] >> (bit & 31)) & 1u) mont_mul_big<L>(acc, acc, vm, M);
+  }
 }
 
 // inverse of the small integer d (1 <= d < 2^32) modulo m, as a plain big number.  false if gcd != 1.
@@ -209,7 +210,7 @@ lagrange_combine_kernel(const LagrangeMod<L> M, const uint32_t k, const int32_t*
         uint32_t t2[L];
 #pragma unroll
         for (int l = 0; l < L; l++) t2[l] = M.m[l];
-        sub_big<L>(t2, lam);
+        limbs::sub<L>(t2, lam);
 #pragma unroll
         for (int l = 0; l < L; l++) lam[l] = t2[l];
       }
@@ -247,7 +248,7 @@ lagrange_combine_kernel(const LagrangeMod<L> M, const uint32_t k, const int32_t*
       S[l] = (uint32_t)v;
       c = v >> 32;
     }
-    if (c || ge_big<L>(S, M.m)) sub_big<L>(S, M.m);
+    if (c || limbs::ge<L>(S, M.m)) limbs::sub<L>(S, M.m);
   }
   uint8_t* ob = out_be + item * (uint64_t)M.mlen;
   for (uint32_t p = 0; p < M.mlen; p++) {

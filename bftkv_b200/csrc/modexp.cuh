@@ -2,14 +2,14 @@
 // "Lagrange in the exponent" steps of the threshold protocols (SURVEY §8f rank 4):
 //   crypto/auth/auth.go:386-399            calculateSharedSecret:  prod_i Y_i^lambda_i mod p
 //   crypto/threshold/dsa/dsa.go:33-52      CalculateR: (prod_i R_i^lambda_i mod p)^((sum v_i lambda_i)^-1 mod q) mod p mod q
-// Reuses K1's lane-distributed radix-2^32 Montgomery product (rsa_verify_r32.cuh): a number is
+// Reuses K1's lane-distributed radix-2^32 Montgomery product (mont_r32.cuh): a number is
 // owned by 4 lanes x W limbs (W = 8: 1024-bit p of DSA L1024; W = 16: the 2048-bit safe prime of
 // crypto/auth).  The modulus must have exactly 128*W bits.  Integer-multiplier bound like K1:
 // one |q|-bit exponentiation = ~1.5 |q| Montgomery products of 2 (4W)^2 MACs.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
-#include "rsa_verify_r32.cuh"
+#include "mont_r32.cuh"
 #include "lagrange.cuh"
 
 namespace bftq {
@@ -21,21 +21,6 @@ struct ModDev {
   uint32_t n0inv;              // -n^-1 mod 2^32
   uint32_t nbytes;             // 16 W
 };
-
-// little-endian 32-bit word k of an nbytes-long big-endian integer
-__device__ __forceinline__ uint32_t be_word_dyn(const uint8_t* p, int nbytes, int k) {
-  const int off = nbytes - 4 - 4 * k;
-  if (off < 0) return 0u;
-  return ((uint32_t)__ldg(p + off) << 24) | ((uint32_t)__ldg(p + off + 1) << 16) | ((uint32_t)__ldg(p + off + 2) << 8) | __ldg(p + off + 3);
-}
-template <int W>
-__device__ __forceinline__ void store_be(uint8_t* p, int nbytes, const uint32_t (&v)[W], int r) {
-#pragma unroll
-  for (int j = 0; j < W; j++) {
-    const int off = nbytes - 4 - 4 * (r * W + j);
-    p[off] = (uint8_t)(v[j] >> 24); p[off + 1] = (uint8_t)(v[j] >> 16); p[off + 2] = (uint8_t)(v[j] >> 8); p[off + 3] = (uint8_t)v[j];
-  }
-}
 
 // out[i] = base[i]^exp[i] mod n.  base: N x nbytes (values >= n are reduced, as big.Int.Exp does),
 // exp: N x elen bytes big-endian.  One 4-lane group per item.
@@ -151,39 +136,17 @@ fermat_inverse_kernel(const LagrangeMod<L> M, const uint8_t* __restrict__ v_be, 
                       uint8_t* __restrict__ status) {
   const uint64_t item = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (item >= n_items) return;
-  uint32_t v[L], e[L], acc[L], vm[L];
-  const uint8_t* vp = v_be + item * (uint64_t)M.mlen;
-#pragma unroll
-  for (int l = 0; l < L; l++) {
-    uint32_t w = 0;
-    for (int b = 0; b < 4; b++) { const int pos = (int)M.mlen - 1 - (4 * l + b); if (pos >= 0) w |= (uint32_t)__ldg(vp + pos) << (8 * b); }
-    v[l] = w; e[l] = M.m[l];
-  }
-  // e = q - 2
-  uint32_t br = 2;
-#pragma unroll
-  for (int l = 0; l < L; l++) { const uint64_t d = (uint64_t)e[l] - br; e[l] = (uint32_t)d; br = (uint32_t)(d >> 63); }
-  bool zero = true;
-#pragma unroll
-  for (int l = 0; l < L; l++) zero = zero && v[l] == 0;
-  while (ge_big<L>(v, M.m)) sub_big<L>(v, M.m);                     // v < 2^(8 mlen) <= 256 q: bounded loop
-  zero = true;
-#pragma unroll
-  for (int l = 0; l < L; l++) zero = zero && v[l] == 0;
-  mont_mul_big<L>(vm, v, M.r2, M);                                  // v R
-#pragma unroll
-  for (int l = 0; l < L; l++) acc[l] = M.r1[l];                     // 1 R
-  for (int bit = 32 * L - 1; bit >= 0; bit--) {
-    mont_mul_big<L>(acc, acc, acc, M);
-    if ((e[bit >> 5] >> (bit & 31)) & 1u) mont_mul_big<L>(acc, acc, vm, M);
-  }
+  uint32_t v[L], acc[L];
+  limbs::load_be<L>(v, v_be + item * (uint64_t)M.mlen, (int)M.mlen);
+  while (limbs::ge<L>(v, M.m)) limbs::sub<L>(v, M.m);               // v < 2^(8 mlen) <= 256 q: bounded loop
+  const bool zero = limbs::is_zero<L>(v);
+  fermat_pow<L>(acc, v, M);
   uint32_t one[L];
 #pragma unroll
   for (int l = 0; l < L; l++) one[l] = 0;
   one[0] = 1;
   mont_mul_big<L>(acc, acc, one, M);
-  uint8_t* ob = out_be + item * (uint64_t)M.mlen;
-  for (uint32_t p = 0; p < M.mlen; p++) { const uint32_t bi = M.mlen - 1 - p; ob[p] = (uint8_t)(acc[bi >> 2] >> (8 * (bi & 3))); }
+  limbs::store_be_bytes<L>(out_be + item * (uint64_t)M.mlen, (int)M.mlen, acc);
   if (zero && status) status[item] = 3;
 }
 
@@ -194,33 +157,9 @@ mod_small_kernel(const LagrangeMod<L> M, const uint8_t* __restrict__ big_be, con
                  uint8_t* __restrict__ out_be) {
   const uint64_t item = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (item >= n_items) return;
-  uint32_t r[L + 1];
-#pragma unroll
-  for (int l = 0; l <= L; l++) r[l] = 0;
-  const uint8_t* bp = big_be + item * (uint64_t)nbytes;
-  for (uint32_t by = 0; by < nbytes; by++) {
-    const uint32_t byte = __ldg(bp + by);
-    for (int bit = 7; bit >= 0; bit--) {
-      // r = 2r + bit ; r < 2q fits L limbs + 1 bit
-      uint32_t c = (byte >> bit) & 1u;
-#pragma unroll
-      for (int l = 0; l <= L; l++) { const uint32_t nc = r[l] >> 31; r[l] = (r[l] << 1) | c; c = nc; }
-      bool ge = r[L] != 0;
-      if (!ge) {
-        ge = true;
-#pragma unroll
-        for (int l = L - 1; l >= 0; l--) { if (r[l] != M.m[l]) { ge = r[l] > M.m[l]; break; } }
-      }
-      if (ge) {
-        uint32_t br = 0;
-#pragma unroll
-        for (int l = 0; l < L; l++) { const uint64_t d = (uint64_t)r[l] - M.m[l] - br; r[l] = (uint32_t)d; br = (uint32_t)(d >> 63); }
-        r[L] -= br;
-      }
-    }
-  }
-  uint8_t* ob = out_be + item * (uint64_t)M.mlen;
-  for (uint32_t p = 0; p < M.mlen; p++) { const uint32_t bi = M.mlen - 1 - p; ob[p] = (uint8_t)(r[bi >> 2] >> (8 * (bi & 3))); }
+  uint32_t r[L];
+  limbs::reduce_be<L>(r, big_be + item * (uint64_t)nbytes, nbytes, M.m);
+  limbs::store_be_bytes<L>(out_be + item * (uint64_t)M.mlen, (int)M.mlen, r);
 }
 
 }  // namespace bftq

@@ -14,7 +14,7 @@
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
-#include "rsa_verify_r32.cuh"
+#include "mont_r32.cuh"
 #include "pgp_digest.cuh"
 
 namespace bftq {
@@ -38,51 +38,6 @@ constexpr uint32_t kDecShort = 2;      // valid padding, message shorter than 3 
 
 using r32::T;
 
-// out = a + b over the 4-lane group, returns the carry out of the top lane (the same in every lane of the group).
-template <int W>
-__device__ __forceinline__ uint32_t ct_add(uint32_t (&out)[W], const uint32_t (&a)[W], const uint32_t (&b)[W], const int r, const int gbase) {
-  uint32_t g;
-  asm volatile("add.cc.u32 %0, %1, %2;" : "=r"(out[0]) : "r"(a[0]), "r"(b[0]));
-#pragma unroll
-  for (int k = 1; k < W; k++) asm volatile("addc.cc.u32 %0, %1, %2;" : "=r"(out[k]) : "r"(a[k]), "r"(b[k]));
-  asm volatile("addc.u32 %0, 0, 0;" : "=r"(g));
-  uint32_t ones = 1u;
-#pragma unroll
-  for (int k = 0; k < W; k++) ones &= (uint32_t)(out[k] == 0xffffffffu);
-  const uint32_t gb = __ballot_sync(kFull, g != 0u) >> gbase;
-  const uint32_t pb = __ballot_sync(kFull, ones != 0u) >> gbase;
-  uint32_t ctop;
-  const uint32_t ci = r32::lane_carry_in(gb, pb, r, ctop);
-  r32::ripple_add(out, ci);
-  return ctop;
-}
-// d = x - n over the group, returns the borrow out of the top lane.
-template <int W>
-__device__ __forceinline__ uint32_t ct_sub(uint32_t (&d)[W], const uint32_t (&x)[W], const uint32_t (&n)[W], const int r, const int gbase) {
-  const uint32_t bo = r32::sub_n(d, x, n);
-  uint32_t zeros = 1u;
-#pragma unroll
-  for (int k = 0; k < W; k++) zeros &= (uint32_t)(d[k] == 0u);
-  const uint32_t bgb = __ballot_sync(kFull, bo != 0u) >> gbase;
-  const uint32_t bpb = __ballot_sync(kFull, zeros != 0u) >> gbase;
-  uint32_t btop;
-  const uint32_t bi = r32::lane_carry_in(bgb, bpb, r, btop);
-  r32::ripple_sub(d, bi);
-  return btop;
-}
-template <int W>
-__device__ __forceinline__ void ct_select(uint32_t (&x)[W], const uint32_t (&y)[W], const uint32_t take_y) {
-  const uint32_t m = 0u - take_y;
-#pragma unroll
-  for (int k = 0; k < W; k++) x[k] = (y[k] & m) | (x[k] & ~m);
-}
-// x -= n when x >= n, masked.
-template <int W>
-__device__ __forceinline__ void ct_cond_sub(uint32_t (&x)[W], const uint32_t (&n)[W], const int r, const int gbase) {
-  uint32_t d[W];
-  const uint32_t bt = ct_sub(d, x, n, r, gbase);
-  ct_select(x, d, bt ^ 1u);
-}
 // A 1024-bit number in the W = 8 layout -> the same number in the W = 16 (2048-bit) layout.
 __device__ __forceinline__ void widen(const uint32_t (&a)[8], uint32_t (&o)[16], const int r, const int gbase) {
   const int s0 = gbase + ((2 * r) & 3), s1 = gbase + ((2 * r + 1) & 3);
@@ -121,49 +76,22 @@ __device__ __forceinline__ void crt_half(uint32_t (&res)[8], const uint32_t (&c_
   make_one(one);
   // c mod m as a value below 2^1024: c_hi * 2^1024 mod m (one product with R^2), + c_lo, minus m while >= 2^1024
   mmul(t, c_hi, r2, m, m0inv, r, gbase);
-  uint32_t hi = ct_add(s, t, c_lo, r, gbase);
+  uint32_t hi = r32::group_add(s, t, c_lo, r, gbase);
 #pragma unroll
   for (int k = 0; k < 2; k++) {
     uint32_t d[W];
-    const uint32_t bt = ct_sub(d, s, m, r, gbase);
-    ct_select(s, d, hi);
+    const uint32_t bt = r32::group_sub(d, s, m, r, gbase);
+    r32::select_mask(s, d, hi);
     hi &= bt ^ 1u;                                // the borrow consumed bit 1024
   }
   uint32_t bm[W];
   mmul(bm, s, r2, m, m0inv, r, gbase);            // Montgomery form of c mod m
   mmul(y, r2, one, m, m0inv, r, gbase);           // Montgomery form of 1
-  const int tid = threadIdx.x;
-#pragma unroll
-  for (int j = 0; j < W; j++) { tab[0][j][tid] = y[j]; tab[1][j][tid] = bm[j]; t[j] = bm[j]; }
-#pragma unroll 1
-  for (int e = 2; e < 16; e++) {
-    uint32_t u[W];
-    mmul(u, t, bm, m, m0inv, r, gbase);
-#pragma unroll
-    for (int j = 0; j < W; j++) { tab[e][j][tid] = u[j]; t[j] = u[j]; }
-  }
-  // fixed-window exponentiation over all 1024 exponent bits, most significant window first
-#pragma unroll 1
-  for (int win = 255; win >= 0; win--) {
-#pragma unroll 1
-    for (int k = 0; k < 4; k++) { mmul(t, y, y, m, m0inv, r, gbase); for (int j = 0; j < W; j++) y[j] = t[j]; }
-    const uint32_t w = (__ldg(dexp + (win >> 3)) >> ((win & 7) * 4)) & 15u;
-    uint32_t sel[W];
-#pragma unroll
-    for (int j = 0; j < W; j++) sel[j] = 0u;
-#pragma unroll
-    for (int e = 0; e < 16; e++) {
-      const uint32_t msk = 0u - (uint32_t)((uint32_t)e == w);
-#pragma unroll
-      for (int j = 0; j < W; j++) sel[j] |= tab[e][j][tid] & msk;
-    }
-    mmul(t, y, sel, m, m0inv, r, gbase);
-#pragma unroll
-    for (int j = 0; j < W; j++) y[j] = t[j];
-  }
+  // fixed-window exponentiation over all 1024 exponent bits
+  r32::ct_window_pow<W, BLOCK>(y, bm, m, m0inv, dexp, 32, 256, tab, r, gbase);
   make_one(one);
   mmul(res, y, one, m, m0inv, r, gbase);          // leaves Montgomery form: <= m
-  ct_cond_sub(res, m, r, gbase);
+  r32::cond_sub<W, true>(res, m, r, gbase);
 }
 
 // One 4-lane group per item.  c_be: n_items x 256 bytes (the PKESK MPI, left-padded; c <= n checked by the host),
@@ -195,21 +123,21 @@ rsa_crt_decrypt_kernel(const RsaPriv32* __restrict__ keys, const uint32_t* __res
     const uint32_t q0inv = __ldg(&key->q0inv);
 #pragma unroll
     for (int j = 0; j < 8; j++) { q[j] = __ldg(key->q + r * 8 + j); uq[j] = __ldg(key->uq + r * 8 + j); a[j] = m1[j]; }
-    ct_cond_sub(a, q, r, gbase);                  // m1 < p < 2q
-    const uint32_t bt = ct_sub(d, m2, a, r, gbase);
+    r32::cond_sub<8, true>(a, q, r, gbase);                 // m1 < p < 2q
+    const uint32_t bt = r32::group_sub(d, m2, a, r, gbase);
     uint32_t dq_[8];
-    ct_add(dq_, d, q, r, gbase);
-    ct_select(d, dq_, bt);
+    r32::group_add(dq_, d, q, r, gbase);
+    r32::select_mask(d, dq_, bt);
     mmul(h, d, uq, q, q0inv, r, gbase);
-    ct_cond_sub(h, q, r, gbase);
+    r32::cond_sub<8, true>(h, q, r, gbase);
     uint32_t h16[16], m16[16], nn[16], pn[16], ph[16], mm[16];
     widen(h, h16, r, gbase);
     widen(m1, m16, r, gbase);
 #pragma unroll
     for (int j = 0; j < 16; j++) { nn[j] = __ldg(key->n + r * 16 + j); pn[j] = __ldg(key->pn + r * 16 + j); }
     mmul(ph, pn, h16, nn, __ldg(&key->n0inv), r, gbase);   // p h mod n, almost reduced
-    ct_cond_sub(ph, nn, r, gbase);
-    ct_add(mm, ph, m16, r, gbase);
+    r32::cond_sub<16, true>(ph, nn, r, gbase);
+    r32::group_add(mm, ph, m16, r, gbase);
     // EM = I2OSP(m, 256) into this group's shared bytes
     uint8_t* em = em_s[grp];
 #pragma unroll

@@ -1,4 +1,4 @@
-// K1's dedicated Montgomery SQUARING (radix 2^32, 4 lanes x 16 limbs) — included by rsa_verify_r32.cuh.
+// K1's dedicated Montgomery SQUARING (radix 2^32, 4 lanes x 16 limbs), on mont_mul's carry chains (mont_r32.cuh).
 //
 // 16 of the 18 Montgomery products of an e = 65537 verification are squarings, and a square needs only half of the
 // limb products a x a of a general product (the n x q half of the CIOS loop stays as it is).  In the lane-distributed
@@ -22,6 +22,7 @@
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
+#include "mont_r32.cuh"
 
 namespace bftq {
 namespace r32 {

@@ -19,22 +19,20 @@
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
+#include "mont_r32.cuh"
 
 namespace bftq {
 
 constexpr int kDigitBits = 28;
 constexpr uint32_t kDigitMask = (1u << kDigitBits) - 1u;
-constexpr int kRsaBytes = 256;       // k = 256: RSA-2048 (the class the fast path and the flat API default to)
-constexpr int kRsaWords = 64;
 constexpr int kMaxDigits = 152;      // digits kept per key (4096-bit class: 8 lanes x 19)
-constexpr int kNumLayouts = 2;       // layout 0 = the class's default (T,W), layout 1 = alternative (2048-bit class only)
 
 // Key-size classes: k = modulus bytes (what Go's pub.Size() returns).  Digit layout per class:
-//   k=128 (1024 bit): 4 lanes x 10 digits    k=192 (1536): 4 x 14    k=256 (2048): 4 x 19 [alt 8 x 10]
+//   k=128 (1024 bit): 4 lanes x 10 digits    k=192 (1536): 4 x 14    k=256 (2048): 4 x 19
 //   k=384 (3072 bit): 8 lanes x 14 digits    k=512 (4096): 8 x 19
 // T*W*28 >= 8k + 24 always, so R > 2^24 n and Montgomery products never need a conditional subtraction.
-__host__ __device__ constexpr int class_digits(int kb, int layout) {
-  return kb == 128 ? 40 : kb == 192 ? 56 : kb == 256 ? (layout == 0 ? 76 : 80) : kb == 384 ? 112 : kb == 512 ? 152 : 0;
+__host__ __device__ constexpr int class_digits(int kb) {
+  return kb == 128 ? 40 : kb == 192 ? 56 : kb == 256 ? 76 : kb == 384 ? 112 : kb == 512 ? 152 : 0;
 }
 __host__ inline bool class_supported(int kb) { return kb == 128 || kb == 192 || kb == 256 || kb == 384 || kb == 512; }
 // Key-size class that carries a modulus of kb = ceil(bits / 8) bytes: the smallest built class that holds it
@@ -45,7 +43,7 @@ __host__ __device__ constexpr int class_of(int kb) { return kb < 1 ? 0 : kb <= 1
 // Per-key constants, precomputed on the host at bftq_register_rsa_keys().
 struct RsaKeyDev {
   uint32_t n[kMaxDigits];                 // modulus, radix 2^28, little-endian digits, zero padded
-  uint32_t r2[kNumLayouts][kMaxDigits];   // R^2 mod n for R = 2^(28*class_digits(kbytes, layout))
+  uint32_t r2[kMaxDigits];                // R^2 mod n for R = 2^(28*class_digits(class_of(kbytes)))
   uint32_t n0inv;                         // -n^-1 mod 2^28
   uint32_t e;                             // public exponent (>= 1)
   uint32_t nbits;
@@ -71,17 +69,7 @@ __host__ inline int host_hash_dlen(uint32_t id) {
   switch (id) { case 1: return 16; case 2: return 20; case 3: return 20; case 8: return 32; case 9: return 48; case 10: return 64; case 11: return 28; default: return 0; }
 }
 
-constexpr unsigned kFull = 0xffffffffu;
-
 // ---- little helpers --------------------------------------------------------------------------
-
-// 32-bit little-endian word k of a KB-byte big-endian integer in global memory.
-template <int KB = kRsaBytes>
-__device__ __forceinline__ uint32_t be_word(const uint8_t* p, int k) {
-  if (k >= KB / 4) return 0u;
-  uint32_t v = __ldg(reinterpret_cast<const uint32_t*>(p + (KB - 4) - 4 * k));
-  return __byte_perm(v, 0, 0x0123);
-}
 
 // Byte i (big-endian position, 0 = most significant) of EMSA-PKCS1-v1_5(digest), k = KB.
 // Mirrors the layout rsa.VerifyPKCS1v15 checks: 00 01 FF.. 00 prefix digest.
@@ -202,15 +190,14 @@ __device__ __forceinline__ void canonicalise(uint32_t (&y)[W], const int r) {
 
 // ---- the kernel -------------------------------------------------------------------------------
 // One group of T lanes per signature; a warp handles 32/T signatures per pass and strides over
-// the batch.  `layout` selects the R^2 table matching T*W digits.
+// the batch.
 template <int T, int W, int BLOCK, int KB>
 __global__ void __launch_bounds__(BLOCK)
 rsa_verify_kernel(const RsaKeyDev* __restrict__ keys, const uint32_t nkeys, const uint32_t* __restrict__ key_idx,
                   const uint8_t* __restrict__ sig, const uint8_t* __restrict__ digest, const uint32_t hash_alg,
                   const uint64_t n_items, const uint32_t flags, const uint8_t* __restrict__ pre_status,
                   uint8_t* __restrict__ status) {
-  constexpr int kLayout = (T * W == class_digits(KB, 0)) ? 0 : 1;
-  static_assert(T * W == class_digits(KB, 0) || T * W == class_digits(KB, 1), "digit layout does not match the key-size class");
+  static_assert(T * W == class_digits(KB), "digit layout does not match the key-size class");
   static_assert(T * W * kDigitBits >= 8 * KB + 24, "R must exceed 2^24 n");
   constexpr int kGroupsPerWarp = 32 / T;
   const int lane = threadIdx.x & 31;
@@ -269,7 +256,7 @@ rsa_verify_kernel(const RsaKeyDev* __restrict__ keys, const uint32_t nkeys, cons
     {
       uint32_t r2[W];
 #pragma unroll
-      for (int j = 0; j < W; j++) r2[j] = __ldg(&key->r2[kLayout][r * W + j]);
+      for (int j = 0; j < W; j++) r2[j] = __ldg(&key->r2[r * W + j]);
       mont_mul<T, W>(xm, xs, r2, nd, n0inv, r, gbase);
     }
     // Left-to-right square and multiply over the bits of e above bit 0.  Control flow is kept

@@ -18,9 +18,9 @@
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
-#include "rsa_verify_r32.cuh"
-#include "modexp.cuh"
-#include "msg_decrypt.cuh"
+#include "mont_r32.cuh"
+#include "limbs.cuh"
+#include "modinv_big.cuh"
 
 namespace bftq {
 namespace k7 {
@@ -60,7 +60,7 @@ thrsa_partial_sign_kernel(const uint64_t* __restrict__ mod_ptr, const uint64_t* 
     const ThrsaMod* __restrict__ M = reinterpret_cast<const ThrsaMod*>(__ldg(mod_ptr + item));
     const uint32_t* __restrict__ fr = reinterpret_cast<const uint32_t*>(__ldg(frag_ptr + item));
     const uint32_t nw = __ldg(frag_words + item);
-    uint32_t nd[W], y[W], t[W], x[W];
+    uint32_t nd[W], y[W], t[W], x[W], bm[W];
 #pragma unroll
     for (int j = 0; j < W; j++) nd[j] = __ldg(&M->n[r * W + j]);
     const uint32_t n0inv = __ldg(&M->n0inv);
@@ -73,53 +73,21 @@ thrsa_partial_sign_kernel(const uint64_t* __restrict__ mod_ptr, const uint64_t* 
 #pragma unroll
       for (int j = 0; j < W; j++) x[j] = (be_word(ip, r * W + j) & msk) | (be_word(mp, r * W + j) & ~msk);
     }
-    // table: entry e = base^e R mod n (almost reduced)
 #pragma unroll
     for (int j = 0; j < W; j++) t[j] = __ldg(&M->r2[r * W + j]);
-    uint32_t bm[W];
     r32::mont_mul<W, true>(bm, x, t, nd, n0inv, r, gbase);
 #pragma unroll
     for (int j = 0; j < W; j++) x[j] = (r == 0 && j == 0) ? 1u : 0u;
     r32::mont_mul<W, true>(y, t, x, nd, n0inv, r, gbase);        // R mod n: the Montgomery form of 1
-#pragma unroll
-    for (int j = 0; j < W; j++) { tab[0][j][tid] = y[j]; tab[1][j][tid] = bm[j]; t[j] = bm[j]; }
-#pragma unroll 1
-    for (int e = 2; e < 16; e++) {
-      r32::mont_mul<W, true>(x, t, bm, nd, n0inv, r, gbase);
-#pragma unroll
-      for (int j = 0; j < W; j++) { tab[e][j][tid] = x[j]; t[j] = x[j]; }
-    }
     // the warp's trip count: the longest fragment of its eight items (public lengths only)
     uint32_t nwmax = nw;
 #pragma unroll
     for (int o = 16; o >= 1; o >>= 1) nwmax = max(nwmax, __shfl_xor_sync(kFull, nwmax, o));
-#pragma unroll 1
-    for (int win = (int)(8u * nwmax) - 1; win >= 0; win--) {
-#pragma unroll 1
-      for (int k = 0; k < 4; k++) {
-        r32::mont_mul<W, true>(t, y, y, nd, n0inv, r, gbase);
-#pragma unroll
-        for (int j = 0; j < W; j++) y[j] = t[j];
-      }
-      const uint32_t wi = (uint32_t)win >> 3;
-      const uint32_t word = wi < nw ? __ldg(fr + 1 + wi) : 0u;
-      const uint32_t w = (word >> ((win & 7) * 4)) & 15u;
-#pragma unroll
-      for (int j = 0; j < W; j++) x[j] = 0u;
-#pragma unroll
-      for (int e = 0; e < 16; e++) {
-        const uint32_t msk = 0u - (uint32_t)((uint32_t)e == w);
-#pragma unroll
-        for (int j = 0; j < W; j++) x[j] |= tab[e][j][tid] & msk;
-      }
-      r32::mont_mul<W, true>(t, y, x, nd, n0inv, r, gbase);
-#pragma unroll
-      for (int j = 0; j < W; j++) y[j] = t[j];
-    }
+    r32::ct_window_pow<W, BLOCK>(y, bm, nd, n0inv, fr + 1, nw, (int)(8u * nwmax), tab, r, gbase);
 #pragma unroll
     for (int j = 0; j < W; j++) x[j] = (r == 0 && j == 0) ? 1u : 0u;
     r32::mont_mul<W, true>(t, y, x, nd, n0inv, r, gbase);         // leaves Montgomery form: <= n
-    k6::ct_cond_sub<W>(t, nd, r, gbase);
+    r32::cond_sub<W, true>(t, nd, r, gbase);
     if (valid) store_be<W>(out_be + item_raw * 256u, 256, t, r);
 #pragma unroll
     for (int e = 0; e < 16; e++)                                  // no power of the base left in shared memory
@@ -130,72 +98,17 @@ thrsa_partial_sign_kernel(const uint64_t* __restrict__ mod_ptr, const uint64_t* 
 }
 
 // ---- m^-1 mod N (public operands) ----------------------------------------------------------------------------------
-__device__ __forceinline__ bool inv_is_zero(const uint32_t* a) {
-  uint32_t o = 0;
-  for (int k = 0; k < 64; k++) o |= a[k];
-  return o == 0;
-}
-__device__ __forceinline__ void inv_shr1(uint32_t* a, uint32_t top) {
-  for (int k = 0; k < 63; k++) a[k] = (a[k] >> 1) | (a[k + 1] << 31);
-  a[63] = (a[63] >> 1) | (top << 31);
-}
-__device__ __forceinline__ uint32_t inv_add(uint32_t* a, const uint32_t* b) {
-  uint64_t c = 0;
-  for (int k = 0; k < 64; k++) { c += (uint64_t)a[k] + b[k]; a[k] = (uint32_t)c; c >>= 32; }
-  return (uint32_t)c;
-}
-__device__ __forceinline__ uint32_t inv_sub(uint32_t* a, const uint32_t* b) {
-  uint64_t br = 0;
-  for (int k = 0; k < 64; k++) { const uint64_t d = (uint64_t)a[k] - b[k] - br; a[k] = (uint32_t)d; br = (d >> 32) & 1u; }
-  return (uint32_t)br;
-}
-__device__ __forceinline__ bool inv_ge(const uint32_t* a, const uint32_t* b) {
-  for (int k = 63; k >= 0; k--) if (a[k] != b[k]) return a[k] > b[k];
-  return true;
-}
-// x / 2 mod n (x < n, n odd)
-__device__ __forceinline__ void inv_half(uint32_t* x, const uint32_t* n) {
-  const uint32_t top = (x[0] & 1u) ? inv_add(x, n) : 0u;
-  inv_shr1(x, top);
-}
-
 // One thread per request: out = m^-1 mod N, bad = 1 when gcd(m, N) != 1 (out zero then).  m < N (an EMSA block).
-// Invariants of the loop: x1 m == u, x2 m == v (mod N).
 __global__ void __launch_bounds__(128)
 thrsa_modinv_kernel(const uint64_t* __restrict__ mod_ptr, const uint8_t* __restrict__ m_be, const uint64_t n_req, uint8_t* __restrict__ out_be,
                     uint8_t* __restrict__ bad) {
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_req) return;
   const ThrsaMod* M = reinterpret_cast<const ThrsaMod*>(mod_ptr[i]);
-  uint32_t n[64], u[64], v[64], x1[64], x2[64];
-  for (int k = 0; k < 64; k++) {
-    n[k] = M->n[k]; v[k] = n[k]; u[k] = be_word(m_be + i * 256u, k);
-    x1[k] = k == 0 ? 1u : 0u; x2[k] = 0u;
-  }
-  bool ok = !inv_is_zero(u);
-  while (ok) {
-    while (!(u[0] & 1u)) { inv_shr1(u, 0u); inv_half(x1, n); }
-    while (!(v[0] & 1u)) { inv_shr1(v, 0u); inv_half(x2, n); }
-    if (inv_ge(u, v)) {
-      inv_sub(u, v);
-      if (inv_sub(x1, x2)) inv_add(x1, n);
-      if (inv_is_zero(u)) break;                 // gcd = v
-    } else {
-      inv_sub(v, u);
-      if (inv_sub(x2, x1)) inv_add(x2, n);
-    }
-  }
-  if (ok) {
-    uint32_t one = v[0] == 1u;
-    for (int k = 1; k < 64; k++) one &= v[k] == 0u;
-    ok = one != 0;
-  }
-  uint8_t* o = out_be + i * 256u;
-  for (int k = 0; k < 64; k++) {
-    const uint32_t w = ok ? x2[k] : 0u;
-    const int off = 256 - 4 - 4 * k;
-    o[off] = (uint8_t)(w >> 24); o[off + 1] = (uint8_t)(w >> 16); o[off + 2] = (uint8_t)(w >> 8); o[off + 3] = (uint8_t)w;
-  }
+  uint32_t n[64], u[64], inv[64];
+  for (int k = 0; k < 64; k++) { n[k] = M->n[k]; u[k] = be_word(m_be + i * 256u, k); }
+  const bool ok = modinv_big<64>(inv, u, n);
+  limbs::store_be_bytes<64>(out_be + i * 256u, 256, inv);
   bad[i] = ok ? 0 : 1;
 }
 

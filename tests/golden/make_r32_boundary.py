@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Boundary moduli and directed operands for the radix-2^32 Montgomery arithmetic (rsa_verify_r32.cuh), seed 0xBF7C0032.
+"""Boundary moduli and directed operands for the radix-2^32 Montgomery arithmetic (mont_r32.cuh), seed 0xBF7C0032.
 Output committed as tests/golden/r32_boundary.json; the tests read it and search for no primes.
 
 Moduli, at 1024 and 2048 bits (and 2047 bits, the radix-2^28 class of K1):

@@ -1,6 +1,6 @@
-"""CPU suite: the radix-2^32 lane-distributed Montgomery arithmetic (rsa_verify_r32.cuh: mont_mul, mont_sqr, mont_finish,
-group_ge, group_sub, cond_sub) on the carry and borrow paths random operands never reach, through its limb emulation
-(tools/emu_r32.py, tools/emu_sq.py, tools/emu_verify.py) at both limb widths, W = 8 (1024-bit numbers: K5, K6a) and
+"""CPU suite: the radix-2^32 lane-distributed Montgomery arithmetic (mont_r32.cuh: mont_mul, mont_finish, group_ge,
+group_sub, cond_sub; rsa_square_r32.cuh: mont_sqr) on the carry and borrow paths random operands never reach, through
+its limb emulation (tools/emu_r32.py, tools/emu_sq.py, tools/emu_verify.py) at both limb widths, W = 8 (1024-bit numbers: K5, K6a) and
 W = 16 (2048-bit numbers: K1, K5).
 
 A carry crosses a lane boundary by propagation only when the whole lane is all ones (mont_finish) or all zeros (the

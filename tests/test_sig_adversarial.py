@@ -4,7 +4,7 @@ CPU only.  The oracle's restatements of Go crypto/ecdsa.Verify and crypto/dsa.Ve
 plain integer restatement; a Python model of ecdsa_verify_core's Shamir ladder shows that each vector reaches the
 branch of pt_add_v it was built for; the host build of the P-256 core (the kernel's own __host__ __device__ code) must
 give the oracle's verdict on every vector; and the host build of modinv_big (dsa_prepare_kernel's s^-1 when q is not
-prime) must agree with pow(s, -1, q)."""
+prime, thrsa_modinv_kernel's m^-1 mod N) must agree with pow(s, -1, q)."""
 import ctypes
 import json
 import os
@@ -278,7 +278,8 @@ def test_p256_core_on_host_matches_oracle(vec, tmp_path):
 
 def test_modinv_on_host(vec, tmp_path):
     """modinv_big from csrc/modinv_big.cuh against pow(s, -1, q): random odd moduli of 3..256 bits, prime and
-    composite, operands sharing a factor with them, and every s of the composite-q DSA rows."""
+    composite, operands sharing a factor with them, and every s of the composite-q DSA rows; and at 64 limbs (K7's
+    m^-1 mod N) random odd 2048-bit moduli and an RSA modulus p q with 0, 1, N - 1 and multiples of p and of q."""
     lib = _build(tmp_path, "libmodinv.so", "modinv_host.cpp")
     out = ctypes.create_string_buffer(32)
 
@@ -308,3 +309,25 @@ def test_modinv_on_host(vec, tmp_path):
     for m in (2 ** 256 - 189, N, P, 3):
         check(rng.randrange(1, m), m)
     assert n > 1000
+
+    # modinv_big<64>: thrsa_modinv_kernel's m^-1 mod N on 2048-bit moduli, random odd ones and the RSA modulus of the
+    # threshold key with operands that share its factor p
+    out64 = ctypes.create_string_buffer(256)
+
+    def check64(a, m):
+        rc = lib.modinv_host64(a.to_bytes(256, "big"), m.to_bytes(256, "big"), out64)
+        if gcd(a, m) == 1:
+            assert rc == 1 and int.from_bytes(out64.raw, "big") == pow(a, -1, m), (a, m)
+        else:
+            assert rc == 0 and out64.raw == bytes(256), (a, m)
+
+    key = json.load(open(os.path.join(HERE, "golden", "thrsa_key.json")))
+    p, q = _h(key["p"]), _h(key["q"])
+    assert p * q == _h(key["n"]) and (p * q).bit_length() == 2048
+    moduli = [rng.getrandbits(2048) | (1 << 2047) | 1 for _ in range(6)] + [p * q]
+    for m in moduli:
+        for a in (0, 1, 2, m - 1, m - 2, rng.randrange(m), 1 << 2046):
+            check64(a, m)
+    for _ in range(4):
+        check64(p * rng.randrange(1, q), p * q)
+        check64(q * rng.randrange(1, p), p * q)

@@ -1,5 +1,5 @@
 """Python emulation of the radix-2^32 lane-distributed Montgomery product of
-bftkv_b200/csrc/rsa_verify_r32.cuh (same E/O/Z/cin bookkeeping), checked against big-int arithmetic.
+bftkv_b200/csrc/mont_r32.cuh (same E/O/Z/cin bookkeeping), checked against big-int arithmetic.
 `owners` < T stops after that many owner steps, as K1's final check does; mont_finish_emu merges the accumulators and
 resolves the carries across the lanes limb for limb (mont_finish), group_sub_emu / cond_sub_emu are group_sub / cond_sub.
 
