@@ -1324,39 +1324,6 @@ int bftq_verify_read_batch(bftq_engine* e, const bftq_quorum* q, const uint32_t*
 }  // extern "C"
 
 namespace {
-template <int L>
-void make_lagrange_mod(const uint8_t* m_be, uint32_t mlen, bftq::LagrangeMod<L>& M) {
-  memset(&M, 0, sizeof(M));
-  for (uint32_t i = 0; i < mlen; i++) {
-    const uint32_t bi = mlen - 1 - i;          // little-endian byte number
-    M.m[bi >> 2] |= (uint32_t)m_be[i] << (8 * (bi & 3));
-  }
-  M.mlen = mlen;
-  M.m0inv = neg_inv32(M.m[0]);
-  // R mod m and R^2 mod m by shift-and-subtract from 1
-  std::vector<uint32_t> r(L + 1, 0u);
-  r[0] = 1;
-  auto ge_m = [&](const std::vector<uint32_t>& v) {
-    if (v[L]) return true;
-    for (int i = L - 1; i >= 0; i--) if (v[i] != M.m[i]) return v[i] > M.m[i];
-    return true;
-  };
-  auto sub_m = [&](std::vector<uint32_t>& v) {
-    uint64_t br = 0;
-    for (int i = 0; i < L; i++) { uint64_t d = (uint64_t)v[i] - M.m[i] - br; v[i] = (uint32_t)d; br = (d >> 63) & 1; }
-    v[L] -= (uint32_t)br;
-  };
-  while (ge_m(r)) sub_m(r);
-  for (int pass = 0; pass < 2; pass++) {
-    for (int b = 0; b < 32 * L; b++) {
-      for (int i = L; i > 0; i--) r[i] = (r[i] << 1) | (r[i - 1] >> 31);
-      r[0] <<= 1;
-      if (ge_m(r)) sub_m(r);
-    }
-    for (int i = 0; i < L; i++) (pass == 0 ? M.r1 : M.r2)[i] = r[i];
-  }
-}
-
 int check_modulus(const uint8_t* m_be, uint32_t mlen) {
   if (mlen == 0 || mlen > 256) return fail(BFTQ_ERR_INVALID_ARG, "modulus length must be 1..256 bytes");
   if (!(m_be[mlen - 1] & 1)) return fail(BFTQ_ERR_INVALID_ARG, "modulus must be odd");
@@ -1371,7 +1338,7 @@ template <int L>
 int launch_lagrange(bftq_engine* e, const uint8_t* m_be, uint32_t mlen, uint32_t k, const int32_t* d_x, const uint8_t* d_y, uint64_t n_items,
                     uint8_t* d_out, uint8_t* d_st, uint8_t* d_lambda, cudaStream_t st) {
   bftq::LagrangeMod<L> M;
-  make_lagrange_mod<L>(m_be, mlen, M);
+  bftq::make_lagrange_mod<L>(m_be, mlen, M);
   const int block = 128;
   bftq::lagrange_combine_kernel<L><<<(unsigned)((n_items + block - 1) / block), block, 0, st>>>(M, k, d_x, d_y, n_items, d_out, d_st, d_lambda);
   CU(cudaGetLastError());
@@ -1582,7 +1549,7 @@ int bftq_dsa_calculate_r_batch(bftq_engine* e, const uint8_t* p_be, uint32_t ple
   // v^-1 mod q (q prime: Fermat)                                    (dsa.go:50)
   {
     bftq::LagrangeMod<8> M;
-    make_lagrange_mod<8>(q_be, qlen, M);
+    bftq::make_lagrange_mod<8>(q_be, qlen, M);
     const int block = 128;
     bftq::fermat_inverse_kernel<8><<<(unsigned)((n_items + block - 1) / block), block, 0, st>>>(M, d_v, n_items, d_vinv, d_st);
     CU(cudaGetLastError());
@@ -1631,7 +1598,7 @@ int bftq_ecdsa_p256_calculate_r_batch(bftq_engine* e, uint32_t k, const int32_t*
   rc = launch_lagrange_any(e, kN, 32, k, d_x, d_vi, n_items, d_v, d_st2, nullptr, st);             // v = sum v_i lambda_i
   if (rc) return rc;
   bftq::LagrangeMod<8> M;
-  make_lagrange_mod<8>(kN, 32, M);
+  bftq::make_lagrange_mod<8>(kN, 32, M);
   bftq::fermat_inverse_kernel<8><<<(unsigned)((n_items + block - 1) / block), block, 0, st>>>(M, d_v, n_items, d_vinv, nullptr);
   CU(cudaGetLastError());
   bftq::p256_sum_mul_kernel<<<(unsigned)((n_items + block - 1) / block), block, 0, st>>>(d_jac, d_ok, k, d_vinv, n_items, d_out, d_st);
@@ -1657,7 +1624,7 @@ int dsa_verify_dev(bftq_engine* e, const uint8_t* p_be, uint32_t plen, const uin
                    const uint8_t* d_r, const uint8_t* d_s, uint32_t stride, const uint8_t* d_dig, uint32_t dlen, uint64_t n,
                    const uint8_t* d_pre, uint8_t* d_u, uint8_t* d_pow, uint8_t* d_prod, uint8_t* d_st, cudaStream_t st) {
   bftq::LagrangeMod<8> M;
-  make_lagrange_mod<8>(q_be, qlen, M);
+  bftq::make_lagrange_mod<8>(q_be, qlen, M);
   const int block = 128;
   const unsigned grid = (unsigned)((n + block - 1) / block);
   bftq::dsa_prepare_kernel<8><<<grid, block, 0, st>>>(M, d_r, d_s, stride, d_dig, dlen, n, d_pre, d_u, d_st);

@@ -14,10 +14,22 @@
 // from a 64-bit extended Euclid — no big-number inversion at all.  Products run in Montgomery form (m must be odd); y_i may be >= m (the
 // reference's big.Int arithmetic reduces it implicitly) as long as it fits mlen bytes.  HBM-bound: k*(4+mlen)+mlen
 // bytes per combine.
+// The per-combine code is __host__ __device__ (tests/harness/lagrange_host.cpp builds it with g++); only the kernel
+// wrapper needs nvcc.
 #pragma once
 #include <cstdint>
+#include <cstring>
+#include <vector>
+#ifdef __CUDACC__
 #include <cuda_runtime.h>
+#define BFTQ_LAG_HD __host__ __device__
+#define BFTQ_LAG_HD_FI __host__ __device__ __forceinline__
+#else
+#define BFTQ_LAG_HD
+#define BFTQ_LAG_HD_FI inline
+#endif
 #include "limbs.cuh"
+#include "bignum_host.hpp"
 
 namespace bftq {
 
@@ -32,7 +44,7 @@ struct LagrangeMod {
 
 // r = a*b*R^-1 mod m, fully reduced.  a < m; b < R.
 template <int L>
-__device__ void mont_mul_big(uint32_t* r, const uint32_t* a, const uint32_t* b, const LagrangeMod<L>& M) {
+BFTQ_LAG_HD void mont_mul_big(uint32_t* r, const uint32_t* a, const uint32_t* b, const LagrangeMod<L>& M) {
   uint32_t t[L + 2];
 #pragma unroll
   for (int i = 0; i < L + 2; i++) t[i] = 0;
@@ -69,7 +81,7 @@ __device__ void mont_mul_big(uint32_t* r, const uint32_t* a, const uint32_t* b, 
 
 // acc = v^(m-2) R mod m (Montgomery form; v^-1 R when m is prime), v < m plain.  Square-and-multiply over all 32 L bits.
 template <int L>
-__device__ __forceinline__ void fermat_pow(uint32_t (&acc)[L], const uint32_t (&v)[L], const LagrangeMod<L>& M) {
+BFTQ_LAG_HD_FI void fermat_pow(uint32_t (&acc)[L], const uint32_t (&v)[L], const LagrangeMod<L>& M) {
   uint32_t e[L], vm[L];
 #pragma unroll
   for (int l = 0; l < L; l++) e[l] = M.m[l];
@@ -87,7 +99,7 @@ __device__ __forceinline__ void fermat_pow(uint32_t (&acc)[L], const uint32_t (&
 
 // inverse of the small integer d (1 <= d < 2^32) modulo m, as a plain big number.  false if gcd != 1.
 template <int L>
-__device__ bool small_inverse(uint32_t* inv, uint32_t d, const LagrangeMod<L>& M) {
+BFTQ_LAG_HD bool small_inverse(uint32_t* inv, uint32_t d, const LagrangeMod<L>& M) {
   if (d == 1) {
 #pragma unroll
     for (int i = 0; i < L; i++) inv[i] = 0;
@@ -132,7 +144,7 @@ __device__ bool small_inverse(uint32_t* inv, uint32_t d, const LagrangeMod<L>& M
 
 // mag mod m as a plain big number (mag < 2^32).
 template <int L>
-__device__ void mag_to_big(uint32_t* out, const uint32_t mag, const LagrangeMod<L>& M) {
+BFTQ_LAG_HD void mag_to_big(uint32_t* out, const uint32_t mag, const LagrangeMod<L>& M) {
 #pragma unroll
   for (int i = 0; i < L; i++) out[i] = 0;
   out[0] = mag;
@@ -142,13 +154,13 @@ __device__ void mag_to_big(uint32_t* out, const uint32_t mag, const LagrangeMod<
   if (tiny) out[0] %= M.m[0];
 }
 
+// One combine: item `item` of the batch (k abscissae at xs + item k, k shares of mlen bytes at ys_be + item k mlen) ->
+// out_be + item mlen, out_status[item] (0, or 3 when a difference has no inverse mod m) and, when out_lambda is not
+// null, the k lambda_i (plain, mlen bytes each) at out_lambda + item k mlen.
 template <int L>
-__global__ void __launch_bounds__(128)
-lagrange_combine_kernel(const LagrangeMod<L> M, const uint32_t k, const int32_t* __restrict__ xs,
-                        const uint8_t* __restrict__ ys_be, const uint64_t n_items, uint8_t* __restrict__ out_be,
-                        uint8_t* __restrict__ out_status, uint8_t* __restrict__ out_lambda) {
-  const uint64_t item = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (item >= n_items) return;
+BFTQ_LAG_HD_FI void lagrange_item(const LagrangeMod<L>& M, const uint32_t k, const int32_t* __restrict__ xs,
+                                  const uint8_t* __restrict__ ys_be, const uint64_t item, uint8_t* __restrict__ out_be,
+                                  uint8_t* __restrict__ out_status, uint8_t* __restrict__ out_lambda) {
   const int32_t* x = xs + item * k;
   const uint8_t* yb = ys_be + item * (uint64_t)k * M.mlen;
   uint32_t S[L];                       // running sum (plain)
@@ -156,7 +168,7 @@ lagrange_combine_kernel(const LagrangeMod<L> M, const uint32_t k, const int32_t*
   for (int i = 0; i < L; i++) S[i] = 0;
   bool okay = true;
   for (uint32_t i = 0; i < k; i++) {
-    const int32_t xi = __ldg(x + i);
+    const int32_t xi = limbs::load_i32(x + i);
     uint32_t lam[L];
 #pragma unroll
     for (int l = 0; l < L; l++) lam[l] = M.r1[l];               // 1 in Montgomery form
@@ -171,7 +183,7 @@ lagrange_combine_kernel(const LagrangeMod<L> M, const uint32_t k, const int32_t*
       const bool last = j == k;
       uint32_t ax = 1u, ad32 = 1u;
       if (!last) {
-        const int32_t xj = __ldg(x + j);
+        const int32_t xj = limbs::load_i32(x + j);
         if (xj == xi) continue;                                  // sss.go:100-102 (also skips duplicates)
         const int64_t d = (int64_t)xj - (int64_t)xi;
         const uint64_t ad = (uint64_t)(d < 0 ? -d : d);
@@ -235,7 +247,7 @@ lagrange_combine_kernel(const LagrangeMod<L> M, const uint32_t k, const int32_t*
 #pragma unroll
       for (int b = 0; b < 4; b++) {
         const int pos = (int)M.mlen - 1 - (4 * l + b);
-        if (pos >= 0) v |= (uint32_t)__ldg(yb + (uint64_t)i * M.mlen + pos) << (8 * b);
+        if (pos >= 0) v |= limbs::load_byte(yb + (uint64_t)i * M.mlen + pos) << (8 * b);
       }
       y[l] = v;
     }
@@ -256,6 +268,52 @@ lagrange_combine_kernel(const LagrangeMod<L> M, const uint32_t k, const int32_t*
     ob[p] = okay ? (uint8_t)(S[byte_index >> 2] >> (8 * (byte_index & 3))) : (uint8_t)0;
   }
   out_status[item] = okay ? 0 : 3;
+}
+
+#ifdef __CUDACC__
+template <int L>
+__global__ void __launch_bounds__(128)
+lagrange_combine_kernel(const LagrangeMod<L> M, const uint32_t k, const int32_t* __restrict__ xs,
+                        const uint8_t* __restrict__ ys_be, const uint64_t n_items, uint8_t* __restrict__ out_be,
+                        uint8_t* __restrict__ out_status, uint8_t* __restrict__ out_lambda) {
+  const uint64_t item = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (item >= n_items) return;
+  lagrange_item<L>(M, k, xs, ys_be, item, out_be, out_status, out_lambda);
+}
+#endif
+
+// Host: the LagrangeMod of the mlen-byte big-endian modulus m_be (odd, > 1, mlen <= 4 L).
+template <int L>
+void make_lagrange_mod(const uint8_t* m_be, uint32_t mlen, LagrangeMod<L>& M) {
+  memset(&M, 0, sizeof(M));
+  for (uint32_t i = 0; i < mlen; i++) {
+    const uint32_t bi = mlen - 1 - i;          // little-endian byte number
+    M.m[bi >> 2] |= (uint32_t)m_be[i] << (8 * (bi & 3));
+  }
+  M.mlen = mlen;
+  M.m0inv = hostbig::neg_inv32(M.m[0]);
+  // R mod m and R^2 mod m by shift-and-subtract from 1
+  std::vector<uint32_t> r(L + 1, 0u);
+  r[0] = 1;
+  auto ge_m = [&](const std::vector<uint32_t>& v) {
+    if (v[L]) return true;
+    for (int i = L - 1; i >= 0; i--) if (v[i] != M.m[i]) return v[i] > M.m[i];
+    return true;
+  };
+  auto sub_m = [&](std::vector<uint32_t>& v) {
+    uint64_t br = 0;
+    for (int i = 0; i < L; i++) { uint64_t d = (uint64_t)v[i] - M.m[i] - br; v[i] = (uint32_t)d; br = (d >> 63) & 1; }
+    v[L] -= (uint32_t)br;
+  };
+  while (ge_m(r)) sub_m(r);
+  for (int pass = 0; pass < 2; pass++) {
+    for (int b = 0; b < 32 * L; b++) {
+      for (int i = L; i > 0; i--) r[i] = (r[i] << 1) | (r[i - 1] >> 31);
+      r[0] <<= 1;
+      if (ge_m(r)) sub_m(r);
+    }
+    for (int i = 0; i < L; i++) (pass == 0 ? M.r1 : M.r2)[i] = r[i];
+  }
 }
 
 }  // namespace bftq

@@ -64,6 +64,13 @@ BFTQ_LIMBS_HD uint32_t load_byte(const uint8_t* p) {
   return *p;
 #endif
 }
+BFTQ_LIMBS_HD int32_t load_i32(const int32_t* p) {
+#ifdef __CUDA_ARCH__
+  return __ldg(p);
+#else
+  return *p;
+#endif
+}
 // v = the nbytes-long big-endian integer at p (its low 4 L bytes when nbytes is larger).
 template <int L>
 BFTQ_LIMBS_HD void load_be(uint32_t (&v)[L], const uint8_t* p, int nbytes) {
