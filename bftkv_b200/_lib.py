@@ -112,6 +112,10 @@ def load():
         "bftq_thrsa_share_destroy": (None, [vp]),
         "bftq_thrsa_sign_batch": (C.c_int, [vp, vp, C.c_uint32, vp, vp, vp, C.c_uint64, vp, vp, C.c_uint64, vp]),
         "bftq_thrsa_process_batch": (C.c_int, [vp, C.c_uint32, C.c_uint32, vp, vp, vp, C.c_uint64, vp, vp, vp, vp, vp, C.c_uint64, vp]),
+        "bftq_thdsa_share_create": (C.c_int, [vp, C.c_uint32, vp, C.c_uint64, C.POINTER(vp)]),
+        "bftq_thdsa_share_destroy": (None, [vp]),
+        "bftq_thdsa_share_out_bound": (C.c_uint64, [vp]),
+        "bftq_thdsa_sign_batch": (C.c_int, [vp, vp, C.c_uint32, vp, vp, vp, vp, C.c_uint64, vp, vp, vp, C.c_uint64, vp, vp, C.c_uint64, vp]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(lib, name)       # AttributeError here = header/library mismatch: fail loudly

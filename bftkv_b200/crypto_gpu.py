@@ -467,3 +467,50 @@ class ThresholdRSA:
         for h in self._shares.values():
             self.engine.thrsa_share_destroy(h)
         self._shares = {}
+
+
+ErrShareNotFound = "crypto: share not found"
+ErrKeyNotFound = "crypto: key not found"
+TH_DSA, TH_ECDSA = 2, 3
+
+
+class ThresholdDSA:
+    """The server half of crypto.Threshold for TH_DSA / TH_ECDSA (crypto/threshold/dsa/dsa_core.go dsaContext.Sign):
+    phases 2 and 3 over registered shares, batched.  Phase 1 (random joint shares, Message.Encrypt) stays on Go, which
+    passes the nonce it kept for the peer.  curve: "dsa" or "p256".  keyring: the server's Keyring (its private key and
+    the nodes' certificates), which decrypts the joint shares."""
+
+    _ERRS = {-8: "threshold dsa: malformed request or share", -13: ErrInvalidInput, -14: ErrShareNotFound, -15: ErrKeyNotFound,
+             -6: ErrInvalidSignature, -9: ErrInvalidTransportSecurityData, -10: ErrMessageBody, -12: ErrMDC, -11: ErrNotBuilt}
+
+    def __init__(self, engine: Engine, curve: str = "dsa"):
+        self.engine = engine
+        self.algo = {"dsa": TH_DSA, "p256": TH_ECDSA}[curve]
+        self._shares = {}
+
+    def register(self, sec: bytes):
+        """Uploads a share once (opt-in: Y and the (k, c) table then live on the device until close())."""
+        if sec not in self._shares:
+            self._shares[sec] = self.engine.thdsa_share_create(self.algo, sec)
+        return self._shares[sec]
+
+    def sign_batch(self, keyring: "Keyring", secs: Sequence[bytes], reqs: Sequence[bytes], peer_ids: Sequence[int], self_id: int,
+                   nonces: Sequence[Optional[bytes]]):
+        """[(serialized partial signature or None, error or None)], as Sign(sec, req, peerId, selfId) returns them, in order."""
+        handles, idx, pos = [], [], {}
+        for s in secs:
+            h = self.register(s)
+            if h.value not in pos:
+                pos[h.value] = len(handles)
+                handles.append(h)
+            idx.append(pos[h.value])
+        err, outs = self.engine.thdsa_sign_batch(keyring._h, handles, idx, list(reqs), list(peer_ids), self_id, list(nonces))
+        return [(o, None) if e == 0 else (None, self._ERRS.get(int(e), ErrDecryptionFailed)) for e, o in zip(err, outs)]
+
+    def sign(self, keyring, sec: bytes, req: bytes, peer_id: int, self_id: int, nonce: Optional[bytes]):
+        return self.sign_batch(keyring, [sec], [req], [peer_id], self_id, [nonce])[0]
+
+    def close(self):
+        for h in self._shares.values():
+            self.engine.thdsa_share_destroy(h)
+        self._shares = {}

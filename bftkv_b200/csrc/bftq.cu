@@ -15,6 +15,7 @@
 #include "msg_parse.cuh"
 #include "msg_decrypt.cuh"
 #include "thrsa_sign.cuh"
+#include "thdsa_sign.cuh"
 #include "pgp_host.hpp"
 #include "wotqs_host.hpp"
 #include "bignum_host.hpp"
@@ -31,6 +32,7 @@
 #include <functional>
 #include <map>
 #include <memory>
+#include <set>
 #include <thread>
 #include <mutex>
 #include <string>
@@ -216,10 +218,14 @@ struct bftq_engine {
   std::vector<bftq_keyring*> keyrings;           // live keyrings: their private-key tables are zeroed at shutdown
   std::mutex thrsa_mu;
   std::vector<bftq_thrsa_share*> thrsa_shares;   // live threshold-RSA shares: their fragments are zeroed at shutdown
+  std::mutex thdsa_mu;                           // threshold-DSA shares and their (k, c) tables
+  std::vector<bftq_thdsa_share*> thdsa_shares;   // live threshold-DSA shares: Y and the tables are zeroed at shutdown
+  uint32_t* d_p256_base = nullptr;               // K8's fixed-base table of P-256 (public), built on first use
 };
 void priv_release(bftq_keyring* kr);             // decrypt_host.inc: zero and free a keyring's private-key table
 void keyring_detach(bftq_keyring* kr);           // a keyring that outlives its engine becomes parse-only
 void thrsa_shutdown(bftq_engine* e);             // thrsa_host.inc: zero and free every live share's fragments
+void thdsa_shutdown(bftq_engine* e);             // thdsa_host.inc: zero and free every live share's Y and (k, c) table
 
 namespace {
 
@@ -690,6 +696,7 @@ void bftq_shutdown(bftq_engine* e) {
     e->keyrings.clear();
   }
   thrsa_shutdown(e);
+  thdsa_shutdown(e);
   for (auto& kv : e->host_allocs) cudaFreeHost(kv.first);
   for (auto* s : e->slots) {
     if (s->stream) { cudaStreamSynchronize(s->stream); cudaStreamDestroy(s->stream); }
@@ -1706,6 +1713,7 @@ int bftq_pgp_digest_batch(bftq_engine* e, const uint8_t* data_blob, const uint64
 #include "packer_host.inc"
 #include "decrypt_host.inc"
 #include "thrsa_host.inc"
+#include "thdsa_host.inc"
 
 // ---- quorum-descriptor builder ------------------------------------------------------------------
 // The descriptor the reference recomputes on EVERY call (client.go:64,101,141,238; server.go:182,211,237,300,473) is a

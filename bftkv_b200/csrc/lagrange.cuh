@@ -43,7 +43,9 @@ struct LagrangeMod {
 };
 
 // r = a*b*R^-1 mod m, fully reduced.  a < m; b < R.
-template <int L>
+// CT: no branch on the data (K8, thdsa_sign.cuh): b's limbs are picked by a masked scan over a public index, so b may
+// live in registers without a local-memory copy, and the final subtraction is always computed and selected with a mask.
+template <int L, bool CT = false>
 BFTQ_LAG_HD void mont_mul_big(uint32_t* r, const uint32_t* a, const uint32_t* b, const LagrangeMod<L>& M) {
   uint32_t t[L + 2];
 #pragma unroll
@@ -51,7 +53,14 @@ BFTQ_LAG_HD void mont_mul_big(uint32_t* r, const uint32_t* a, const uint32_t* b,
 #pragma unroll 1
   for (int i = 0; i < L; i++) {
     uint64_t c = 0;
-    const uint32_t bi = b[i];
+    uint32_t bi;
+    if (CT) {
+      bi = 0u;
+#pragma unroll
+      for (int k = 0; k < L; k++) bi |= b[k] & (0u - (uint32_t)(k == i));
+    } else {
+      bi = b[i];
+    }
 #pragma unroll
     for (int j = 0; j < L; j++) {
       const uint64_t v = (uint64_t)a[j] * bi + t[j] + c;
@@ -74,7 +83,17 @@ BFTQ_LAG_HD void mont_mul_big(uint32_t* r, const uint32_t* a, const uint32_t* b,
     t[L - 1] = (uint32_t)v;
     t[L] = t[L + 1] + (uint32_t)(v >> 32);
   }
-  if (t[L] != 0 || limbs::ge<L>(t, M.m)) limbs::sub<L>(t, M.m);
+  if (CT) {
+    uint32_t d[L];
+    uint32_t br = 0;
+#pragma unroll
+    for (int i = 0; i < L; i++) { const uint64_t x = (uint64_t)t[i] - M.m[i] - br; d[i] = (uint32_t)x; br = (uint32_t)(x >> 63); }
+    const uint32_t take = 0u - ((uint32_t)(t[L] != 0u) | (br ^ 1u));      // t >= m (t < 2m)
+#pragma unroll
+    for (int i = 0; i < L; i++) t[i] = (d[i] & take) | (t[i] & ~take);
+  } else if (t[L] != 0 || limbs::ge<L>(t, M.m)) {
+    limbs::sub<L>(t, M.m);
+  }
 #pragma unroll
   for (int i = 0; i < L; i++) r[i] = t[i];
 }

@@ -300,6 +300,189 @@ BFTQ_P_HD bool ecdsa_verify_core(const pt& q, const uint32_t (&r)[8], const uint
   return fe_eq(x, r);
 }
 
+// ---- constant time: a * G for a secret a (K8, thdsa_sign.cuh) -------------------------------------
+// Masked variants of fe_add / fe_sub / fe_mul: the final correction is always computed and selected with a mask, every
+// loop has a fixed trip count, and everything is forced inline so no field element is ever addressed in local memory.
+#ifdef __CUDACC__
+#define BFTQ_P_CT __host__ __device__ __forceinline__
+#else
+#define BFTQ_P_CT inline
+#endif
+
+BFTQ_P_CT void fe_select(fe r, const fe a, const uint32_t take_a) {     // r = take_a ? a : r  (take_a 0 / 1)
+  const uint32_t m = 0u - take_a;
+#pragma unroll
+  for (int i = 0; i < 8; i++) r[i] = (a[i] & m) | (r[i] & ~m);
+}
+BFTQ_P_CT void fe_add_ct(fe r, const fe a, const fe b) {
+  const uint32_t P[8] = BFTQ_P256_P;
+  uint32_t t[8], d[8], c = 0, br = 0;
+#pragma unroll
+  for (int i = 0; i < 8; i++) { const uint64_t v = (uint64_t)a[i] + b[i] + c; t[i] = (uint32_t)v; c = (uint32_t)(v >> 32); }
+#pragma unroll
+  for (int i = 0; i < 8; i++) { const uint64_t v = (uint64_t)t[i] - P[i] - br; d[i] = (uint32_t)v; br = (uint32_t)(v >> 63); }
+  const uint32_t take = 0u - (c | (br ^ 1u));                    // a + b >= p
+#pragma unroll
+  for (int i = 0; i < 8; i++) r[i] = (d[i] & take) | (t[i] & ~take);
+}
+BFTQ_P_CT void fe_sub_ct(fe r, const fe a, const fe b) {
+  const uint32_t P[8] = BFTQ_P256_P;
+  uint32_t t[8], br = 0, c = 0;
+#pragma unroll
+  for (int i = 0; i < 8; i++) { const uint64_t v = (uint64_t)a[i] - b[i] - br; t[i] = (uint32_t)v; br = (uint32_t)(v >> 63); }
+  const uint32_t m = 0u - br;                                    // a < b: add p back
+#pragma unroll
+  for (int i = 0; i < 8; i++) { const uint64_t v = (uint64_t)t[i] + (P[i] & m) + c; r[i] = (uint32_t)v; c = (uint32_t)(v >> 32); }
+}
+// Montgomery product a*b/R mod p as fe_mul_v, with the final subtraction masked
+BFTQ_P_CT void fe_mul_ct(fe r, const fe a, const fe b) {
+  const uint32_t P[8] = BFTQ_P256_P;
+  uint32_t t[10];
+#pragma unroll
+  for (int i = 0; i < 10; i++) t[i] = 0;
+#pragma unroll
+  for (int i = 0; i < 8; i++) {
+    uint64_t c = 0;
+#pragma unroll
+    for (int j = 0; j < 8; j++) { const uint64_t v = (uint64_t)a[j] * b[i] + t[j] + c; t[j] = (uint32_t)v; c = v >> 32; }
+    uint64_t v = (uint64_t)t[8] + c; t[8] = (uint32_t)v; t[9] = (uint32_t)(v >> 32);
+    const uint32_t q = t[0];
+    v = (uint64_t)q * P[0] + t[0]; c = v >> 32;
+#pragma unroll
+    for (int j = 1; j < 8; j++) { v = (uint64_t)q * P[j] + t[j] + c; t[j - 1] = (uint32_t)v; c = v >> 32; }
+    v = (uint64_t)t[8] + c; t[7] = (uint32_t)v; t[8] = t[9] + (uint32_t)(v >> 32);
+  }
+  uint32_t d[8], br = 0;
+#pragma unroll
+  for (int i = 0; i < 8; i++) { const uint64_t v = (uint64_t)t[i] - P[i] - br; d[i] = (uint32_t)v; br = (uint32_t)(v >> 63); }
+  const uint32_t take = 0u - ((uint32_t)(t[8] != 0u) | (br ^ 1u));
+#pragma unroll
+  for (int i = 0; i < 8; i++) r[i] = (d[i] & take) | (t[i] & ~take);
+}
+// a^(p-2): the exponent is the public constant p - 2, so the square-and-multiply pattern reveals nothing; 0 maps to 0.
+BFTQ_P_CT void fe_inv_ct(fe r, const fe a) {
+  const uint32_t R1[8] = BFTQ_P256_R1;
+  fe acc;
+#pragma unroll
+  for (int i = 0; i < 8; i++) acc[i] = R1[i];
+#pragma unroll 1
+  for (int bit = 255; bit >= 0; bit--) {
+    fe_mul_ct(acc, acc, acc);
+    const int wi = bit >> 5;                                     // word wi of p - 2, without an indexed array
+    const uint32_t e = (wi == 7 || wi == 2 || wi == 1) ? 0xffffffffu : wi == 6 ? 1u : wi == 0 ? 0xfffffffdu : 0u;
+    if ((e >> (bit & 31)) & 1u) fe_mul_ct(acc, acc, a);
+  }
+#pragma unroll
+  for (int i = 0; i < 8; i++) r[i] = acc[i];
+}
+
+// Homogeneous projective point (X : Y : Z), x = X / Z, y = Y / Z, Montgomery form; the identity is (0 : 1 : 0).
+struct ppt { fe X, Y, Z; };
+
+// Complete addition for a = -3 (Renes, Costello, Batina, "Complete addition formulas for prime order elliptic curves",
+// EUROCRYPT 2016, Algorithm 4): one straight-line sequence for every pair of inputs, doublings and the identity included.
+BFTQ_P_CT void ppt_add_ct(ppt& o, const ppt& p, const ppt& q) {
+  const uint32_t BM[8] = BFTQ_P256_BM;
+  fe t0, t1, t2, t3, t4, X3, Y3, Z3;
+  fe_mul_ct(t0, p.X, q.X); fe_mul_ct(t1, p.Y, q.Y); fe_mul_ct(t2, p.Z, q.Z);
+  fe_add_ct(t3, p.X, p.Y); fe_add_ct(t4, q.X, q.Y); fe_mul_ct(t3, t3, t4);
+  fe_add_ct(t4, t0, t1); fe_sub_ct(t3, t3, t4); fe_add_ct(t4, p.Y, p.Z);
+  fe_add_ct(X3, q.Y, q.Z); fe_mul_ct(t4, t4, X3); fe_add_ct(X3, t1, t2);
+  fe_sub_ct(t4, t4, X3); fe_add_ct(X3, p.X, p.Z); fe_add_ct(Y3, q.X, q.Z);
+  fe_mul_ct(X3, X3, Y3); fe_add_ct(Y3, t0, t2); fe_sub_ct(Y3, X3, Y3);
+  fe_mul_ct(Z3, BM, t2); fe_sub_ct(X3, Y3, Z3); fe_add_ct(Z3, X3, X3);
+  fe_add_ct(X3, X3, Z3); fe_sub_ct(Z3, t1, X3); fe_add_ct(X3, t1, X3);
+  fe_mul_ct(Y3, BM, Y3); fe_add_ct(t1, t2, t2); fe_add_ct(t2, t1, t2);
+  fe_sub_ct(Y3, Y3, t2); fe_sub_ct(Y3, Y3, t0); fe_add_ct(t1, Y3, Y3);
+  fe_add_ct(Y3, t1, Y3); fe_add_ct(t1, t0, t0); fe_add_ct(t0, t1, t0);
+  fe_sub_ct(t0, t0, t2); fe_mul_ct(t1, t4, Y3); fe_mul_ct(t2, t0, Y3);
+  fe_mul_ct(Y3, X3, Z3); fe_add_ct(Y3, Y3, t2); fe_mul_ct(X3, t3, X3);
+  fe_sub_ct(X3, X3, t1); fe_mul_ct(Z3, t4, Z3); fe_mul_ct(t1, t3, t0);
+  fe_add_ct(Z3, Z3, t1);
+#pragma unroll
+  for (int i = 0; i < 8; i++) { o.X[i] = X3[i]; o.Y[i] = Y3[i]; o.Z[i] = Z3[i]; }
+}
+
+// The fixed-base table: entry (i, j) = (j + 1) 16^i G for window i = 0..63 and digit j + 1 = 1..15, affine X then Y in
+// Montgomery form, 16 words per entry.  Public data, built once per engine by p256_base_table.
+constexpr int kBaseWindows = 64, kBaseDigits = 15, kBaseEntryWords = 16;
+constexpr int kBaseTableWords = kBaseWindows * kBaseDigits * kBaseEntryWords;
+
+BFTQ_P_CT uint32_t base_tab_word(const uint32_t* tab, int k) {
+#ifdef __CUDA_ARCH__
+  return __ldg(tab + k);
+#else
+  return tab[k];
+#endif
+}
+
+// out65 = elliptic.Marshal(a G) for a scalar a < 2^256 (8 little-endian words): 04 || x || y, and 04 || 0^64 when a G is
+// the identity (a = 0 mod N).  One complete addition per 4-bit window, each reading all fifteen entries of its row with
+// masks; the affine conversion inverts Z with the fixed exponent p - 2, which maps Z = 0 to 0 and so the identity to
+// (0, 0) without a branch.
+BFTQ_P_CT void base_mul_ct(uint8_t* out65, const uint32_t (&a)[8], const uint32_t* tab) {
+  const uint32_t R1[8] = BFTQ_P256_R1;
+  ppt acc;
+#pragma unroll
+  for (int i = 0; i < 8; i++) { acc.X[i] = 0u; acc.Y[i] = R1[i]; acc.Z[i] = 0u; }
+#pragma unroll 1
+  for (int w = 0; w < kBaseWindows; w++) {
+    uint32_t word = 0u;                                          // a's word w / 8, by a masked scan (a stays in registers)
+#pragma unroll
+    for (int k = 0; k < 8; k++) word |= a[k] & (0u - (uint32_t)(k == (w >> 3)));
+    const uint32_t d = (word >> (4 * (w & 7))) & 15u;
+    ppt s;
+#pragma unroll
+    for (int i = 0; i < 8; i++) { s.X[i] = 0u; s.Y[i] = 0u; }
+    const uint32_t* row = tab + w * kBaseDigits * kBaseEntryWords;
+#pragma unroll 1
+    for (int j = 0; j < kBaseDigits; j++) {
+      const uint32_t m = 0u - (uint32_t)((uint32_t)(j + 1) == d);
+#pragma unroll
+      for (int i = 0; i < 8; i++) {
+        s.X[i] |= base_tab_word(row, j * kBaseEntryWords + i) & m;
+        s.Y[i] |= base_tab_word(row, j * kBaseEntryWords + 8 + i) & m;
+      }
+    }
+    const uint32_t zero = 0u - (uint32_t)(d == 0u);              // digit 0: the identity (0 : 1 : 0)
+#pragma unroll
+    for (int i = 0; i < 8; i++) { s.Y[i] |= R1[i] & zero; s.Z[i] = R1[i] & ~zero; }
+    ppt t;
+    ppt_add_ct(t, acc, s);
+    acc = t;
+  }
+  fe zi, x, y;
+  const uint32_t one[8] = {1, 0, 0, 0, 0, 0, 0, 0};
+  fe_inv_ct(zi, acc.Z);
+  fe_mul_ct(x, acc.X, zi); fe_mul_ct(y, acc.Y, zi);
+  fe_mul_ct(x, x, one); fe_mul_ct(y, y, one);
+  out65[0] = 4;
+  limbs_to_be(out65 + 1, x);
+  limbs_to_be(out65 + 33, y);
+}
+
+// Host: the table base_mul_ct reads (kBaseTableWords words), with the variable-time arithmetic above: G is public.
+inline void base_table(uint32_t* tab) {
+  const uint32_t R1[8] = BFTQ_P256_R1;
+  const uint32_t GX[8] = BFTQ_P256_GXM;
+  const uint32_t GY[8] = BFTQ_P256_GYM;
+  pt b;                                                          // 16^i G
+  fe_set(b.X, GX); fe_set(b.Y, GY); fe_set(b.Z, R1);
+  for (int w = 0; w < kBaseWindows; w++) {
+    pt m = b;
+    for (int j = 0; j < kBaseDigits; j++) {
+      uint8_t xb[32], yb[32];
+      uint32_t xw[8], yw[8];
+      pt_to_affine(xb, yb, m);
+      be_to_limbs(xw, xb); be_to_limbs(yw, yb);
+      uint32_t* e = tab + (w * kBaseDigits + j) * kBaseEntryWords;
+      fe_to_mont(e, xw); fe_to_mont(e + 8, yw);
+      pt_add(m, m, b);
+    }
+    for (int k = 0; k < 4; k++) pt_dbl(b, b);
+  }
+}
+
 }}  // namespace bftq::p256
 
 #ifdef __CUDACC__

@@ -326,6 +326,35 @@ class Engine:
         return [(int(state[p]), int(err[p]), int(at[p]), bytes(sig[p]) if state[p] == 1 else None,
                  [int(x) for x in miss[moff[p]:moff[p + 1]]]) for p in range(P)]
 
+    # ---- K8: threshold DSA / ECDSA partial signing (crypto/threshold/dsa/dsa_core.go) ----
+    def thdsa_share_create(self, algo: int, sec: bytes):
+        """Registers one share (dsaContext's saved parameter; algo 2 = TH_DSA, 3 = TH_ECDSA) on the device; returns its handle."""
+        h = C.c_void_p()
+        buf = np.frombuffer(sec, np.uint8) if sec else np.zeros(1, np.uint8)
+        _lib.check(self._lib.bftq_thdsa_share_create(self._h, algo, _ptr(buf), len(sec), C.byref(h)))
+        return h
+
+    def thdsa_share_destroy(self, share):
+        self._lib.bftq_thdsa_share_destroy(share)
+
+    def thdsa_sign_batch(self, keyring, shares, share_idx, requests, peer_ids, self_id: int, nonces):
+        """dsaContext.Sign phases 2 / 3 over (shares[share_idx[i]], requests[i], peer_ids[i]); nonces[i]: the phase-1 nonce
+        stored for the peer, or None.  keyring: a crypto_gpu.Keyring handle.  (out_err int32[n], [serialized outputs])."""
+        n = len(requests)
+        blob, off = self._blob(list(requests))
+        nblob, noff = self._blob([x or b"" for x in nonces])
+        has = np.array([x is not None for x in nonces] or [0], np.uint8)
+        tab = (C.c_void_p * max(1, len(shares)))(*[s.value for s in shares])
+        idx = np.ascontiguousarray(share_idx, np.uint32)
+        peers = np.ascontiguousarray(peer_ids, np.uint64) if n else np.zeros(1, np.uint64)
+        cap = sum(int(self._lib.bftq_thdsa_share_out_bound(shares[i])) for i in share_idx)
+        out = np.zeros(max(1, cap), np.uint8)
+        out_off = np.zeros(n + 1, np.uint64)
+        err = np.zeros(max(1, n), np.int32)
+        _lib.check(self._lib.bftq_thdsa_sign_batch(keyring, tab, len(shares), _ptr(idx), _ptr(blob), _ptr(off), _ptr(peers), self_id,
+                                                   _ptr(nblob), _ptr(noff), _ptr(has), n, _ptr(err), _ptr(out), cap, _ptr(out_off)))
+        return err[:n], [bytes(out[out_off[i]:out_off[i + 1]]) for i in range(n)]
+
     def lagrange_exp_product_batch(self, p: int, q: int, x, ys):
         """auth.calculateSharedSecret: prod_j ys[i][j]^lambda_j mod p.  x: (B,k) ints, ys: B lists of k ints."""
         plen, qlen = (p.bit_length() + 7) // 8, (q.bit_length() + 7) // 8

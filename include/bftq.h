@@ -48,6 +48,8 @@ extern "C" {
 #define BFTQ_ERR_UNSUPPORTED      -11   /* a form the reference's library handles and this build does not (compressed data)       */
 #define BFTQ_ERR_MDC             -12   /* the SEIPD packet's modification detection code does not match: ReadAll's error, returned as is */
 #define BFTQ_ERR_INVALID_INPUT   -13   /* crypto.ErrInvalidInput (threshold RSA: the hash info leaves less than 3 padding bytes) */
+#define BFTQ_ERR_SHARE_NOT_FOUND -14   /* crypto.ErrShareNotFound (threshold DSA: no joint share for this node, or a stale nonce) */
+#define BFTQ_ERR_KEY_NOT_FOUND   -15   /* crypto.ErrKeyNotFound (threshold DSA: phase 3 without a phase 2 for the peer) */
 
 /* ---- per-item status bytes (SURVEY §8b "Errors") --------------------------------------------
  * The reference collapses every failure to ErrInvalidSignature (crypto_pgp.go:325-327); the shim
@@ -354,6 +356,48 @@ int bftq_thrsa_sign_batch(bftq_engine* e, bftq_thrsa_share* const* shares, uint3
 int bftq_thrsa_process_batch(bftq_engine* e, uint32_t n, uint32_t k, const uint8_t* resp_blob, const uint64_t* resp_off,
                              const uint64_t* proc_off, uint64_t n_procs, int32_t* out_state, int32_t* out_err, uint64_t* out_at,
                              uint8_t* out_sig, uint32_t* out_missing, uint64_t missing_cap, uint64_t* out_missing_off);
+/* ---- K8: threshold DSA / ECDSA partial signing (crypto/threshold/dsa/dsa_core.go:91-163 dsaContext.Sign) ------------
+ * A share is dsaContext's saved parameter: the bytes of ThresholdInstance's secret after its algo byte, whose value
+ * (crypto.TH_DSA = 2, TH_ECDSA = 3) is `algo`.  serializePartialParam's framing: the group (DSA: chunks p, q, g; ECDSA:
+ * chunks P, N, B, Gx, Gy and a u32 BitSize), then u64 X, the chunk Y, u16 t and the nodes' OpenPGP entity stream.
+ * Registration is opt-in: Y goes to one device allocation per share, zeroed before it is freed (bftq_thdsa_share_destroy,
+ * bftq_shutdown), and the host copy is wiped after upload.  The entity stream is read leniently (it serves phase 1 only):
+ * a stream Go's ParseStream rejects does not fail registration here.
+ *   BFTQ_ERR_MALFORMED        framing error (truncated share)
+ *   BFTQ_ERR_UNSUPPORTED_KEY  DSA without p odd of exactly 1024 / 2048 bits and q odd of 33..256 bits, or an ECDSA group
+ *                             that is not exactly P-256 (P, N, B, Gx, Gy, BitSize 256): the shim keeps such a share on Go */
+#define BFTQ_THDSA_DSA   2
+#define BFTQ_THDSA_ECDSA 3
+typedef struct bftq_thdsa_share bftq_thdsa_share;
+typedef struct bftq_keyring bftq_keyring;          /* the packet-level keyring, below */
+int bftq_thdsa_share_create(bftq_engine* e, uint32_t algo, const uint8_t* sec, uint64_t len, bftq_thdsa_share** out);
+void bftq_thdsa_share_destroy(bftq_thdsa_share* s);
+/* The most bytes one item signed with this share can write: 8 + (8 + |p| or 65) + (8 + 32) + the group's serialized length. */
+uint64_t bftq_thdsa_share_out_bound(const bftq_thdsa_share* s);
+/* dsaContext.Sign's phases 2 and 3 over n_items requests.  Item i: request req_blob[req_off[i] .. req_off[i+1]) for share
+ * shares[share_idx[i]] from client peer_id[i]; self_id is this server's node id.  has_nonce[i] / nonce_blob[nonce_off[i] ..
+ * nonce_off[i+1]): the nonce phase 1 (on Go) stored for peer_id[i], ctx.nonces[peerId].  The items behave as if they ran one
+ * after another in item order: a phase-3 item uses the (k_i, c_i) of the latest earlier phase-2 item for the same (share,
+ * peer), in this call or an earlier one; the share's table of them grows as Go's map does and is never evicted.  Every
+ * encrypted share of every phase-2 item is decrypted in ONE bftq_message_decrypt_batch on `kr`, which holds this server's
+ * private key and the nodes' certificates.
+ * Output: item i's serializePartialSignature bytes at out_blob[out_off[i] .. out_off[i+1]), packed.  Phase 2: u64 x,
+ * chunk(R_i), chunk(v_i), the group; phase 3: u64 X, chunk(s_i), an empty chunk, the group.  R_i: DSA g^{a_i} mod p minimal
+ * (01 for a_i = 0), ECDSA elliptic.Marshal(a_i G) (04 || 0^64 for a_i = 0).  out_cap must hold the sum over items of
+ * bftq_thdsa_share_out_bound(their share), else BFTQ_ERR_INVALID_ARG before any work.
+ *   out_err[i]  0 | BFTQ_ERR_MALFORMED (request framing; a share message's framing; a share whose signer key id is not the
+ *               primary key id of an entity in the keyring, where GetCertById returns nil and Go panics on signer.Id(); or,
+ *               as bftq_message_decrypt_batch reports it, a share message ReadMessage cannot read, which Go returns as
+ *               crypto.ErrDecryptionFailed: the code does not tell these apart) | BFTQ_ERR_SHARE_NOT_FOUND (no entry for self_id,
+ *               no self-signed share, or its nonce differs from / lacks the stored one) | BFTQ_ERR_INVALID_INPUT (the four
+ *               X of a share differ from the first share's X, or the entry for self_id holds no share) |
+ *               BFTQ_ERR_KEY_NOT_FOUND (phase 3 without a phase 2) | a code of bftq_message_decrypt_batch for the first share
+ *               that fails, as Message.Decrypt returns it; BFTQ_ERR_UNSUPPORTED there means: run this Sign on Go, and route
+ *               the (share, peer)'s phase 3 to Go too.  A failed item stores nothing. */
+int bftq_thdsa_sign_batch(bftq_keyring* kr, bftq_thdsa_share* const* shares, uint32_t n_shares, const uint32_t* share_idx,
+                          const uint8_t* req_blob, const uint64_t* req_off, const uint64_t* peer_id, uint64_t self_id,
+                          const uint8_t* nonce_blob, const uint64_t* nonce_off, const uint8_t* has_nonce, uint64_t n_items,
+                          int32_t* out_err, uint8_t* out_blob, uint64_t out_cap, uint64_t* out_off);
 /* AuthClient.calculateSharedSecret (crypto/auth/auth.go:386-399) and the first half of CalculateR:
  * out[i] = prod_j y[i][j]^lambda_j mod p,  lambda_j = sss.Lagrange(x[i][j], x[i][*], q).
  * p: plen = 128/256 bytes; q: any odd modulus up to 256 bytes (auth uses q = (p-1)/2). */
