@@ -514,3 +514,71 @@ class ThresholdDSA:
         for h in self._shares.values():
             self.engine.thdsa_share_destroy(h)
         self._shares = {}
+
+
+ErrAuthenticationFailure = "authentication failure"
+ErrAuthTooManyAttempts = "crypto: too many attempts"
+AUTH_RETRY_LIMIT = 10
+AUTH_DELAY_RATE = 1.0                  # seconds of delay per earlier phase-0 attempt (auth.go AUTH_DELAY_RATE)
+# p of crypto/auth (auth.go:81-115)
+AUTH_P = int("b0a67d9f5cebc0ffe81690e7b2670ab05f9fa4c2e73639f660c0408a2d9a4a8b454a9893fd7d4e8fa399cfc9c9ba05b080f903e33bcdcbefaed40915"
+             "e51d46f58d1a5bd204db20fa3fe9db71f0b8e0aa87b5771406f25fad59e7f10fe52556447588"
+             "72ea2dec1f6dcd11be905de59a044f6c2ea3982b2235acc9021a196fc4ce0b19f6b312ee9cfc5997dc5f7ce2f386131294a56ba93a41a3b60e27e03956039f51"
+             "ae73b89c795c5ae7d841e9b455c37341c052404e8fe9fe4f0d52bc162a41f1eeb9ef292c66a9d6a619aa548807eb1187ee22bd62e20e26c3c08c22ecef12d3"
+             "b2304a010ed1f50a68e0261afe1a0bdddf7ab8a61774d3af3f1cce2b95dad3", 16)
+
+
+class AuthServer:
+    """The server half of crypto/auth (threshold password authentication): NewServer / MakeResponse over a server
+    registered on the device.  Phase 0 answers Yi, phase 1 Bi (and keeps ke and the MAC on the device), phase 2 seals the
+    proof.  The attempts counter and its delay stay here, as in auth.go; `delay` is the sleep function (injectable, so
+    tests do not sleep).  One divergence: phase 2 before any phase 1 is ErrAuthenticationFailure (the reference seals the
+    proof under an all-zero key there)."""
+
+    def __init__(self, engine: Engine, params: bytes, proof: bytes, delay=None):
+        import time
+        self.engine = engine
+        self.attempts = 0
+        self._delay = delay if delay is not None else time.sleep
+        self._h = engine.auth_server_create(params, proof)
+
+    @staticmethod
+    def draw(phase: int) -> bytes:
+        """The randomness MakeResponse draws: b = rand.Int(rand.Reader, p) for phase 1, a 12-byte nonce for phase 2."""
+        import secrets
+        if phase == 1:
+            return secrets.randbelow(AUTH_P).to_bytes(256, "big")
+        return secrets.token_bytes(12) if phase == 2 else b""
+
+    @classmethod
+    def respond_batch(cls, engine: Engine, servers: Sequence["AuthServer"], phases: Sequence[int], reqs: Sequence[bytes],
+                      rands: Optional[Sequence[bytes]] = None):
+        """MakeResponse over distinct servers in one call: [(res, done, err)] in order.  rands: the randomness per item
+        (None: drawn here)."""
+        if rands is None:
+            rands = [cls.draw(p) for p in phases]
+        err, outs = engine.auth_server_respond_batch([s._h for s in servers], list(range(len(servers))), list(phases), list(reqs), list(rands))
+        res = []
+        for s, ph, e, o in zip(servers, phases, err, outs):
+            if ph == 0:
+                delay = s.attempts * AUTH_DELAY_RATE
+                if delay > 0:
+                    s._delay(delay)
+                s.attempts += 1
+                res.append((o, False, ErrAuthTooManyAttempts if s.attempts >= AUTH_RETRY_LIMIT else None))
+            elif ph == 1:
+                res.append((o, False, None))
+            elif ph == 2:
+                res.append((o, True, None) if e == 0 else (None, True, ErrAuthenticationFailure))
+            else:
+                res.append((None, False, None))
+        return res
+
+    def make_response(self, phase: int, req: bytes, rand: Optional[bytes] = None):
+        """(res, done, err) as AuthServer.MakeResponse returns them."""
+        return self.respond_batch(self.engine, [self], [phase], [req], None if rand is None else [rand])[0]
+
+    def close(self):
+        if self._h is not None:
+            self.engine.auth_server_destroy(self._h)
+            self._h = None

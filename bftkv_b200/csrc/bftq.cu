@@ -16,6 +16,7 @@
 #include "msg_decrypt.cuh"
 #include "thrsa_sign.cuh"
 #include "thdsa_sign.cuh"
+#include "auth_server.cuh"
 #include "pgp_host.hpp"
 #include "wotqs_host.hpp"
 #include "bignum_host.hpp"
@@ -221,11 +222,15 @@ struct bftq_engine {
   std::mutex thdsa_mu;                           // threshold-DSA shares and their (k, c) tables
   std::vector<bftq_thdsa_share*> thdsa_shares;   // live threshold-DSA shares: Y and the tables are zeroed at shutdown
   uint32_t* d_p256_base = nullptr;               // K8's fixed-base table of P-256 (public), built on first use
+  std::mutex auth_mu;                            // password-authentication servers and the calls that use them
+  std::vector<bftq_auth_server*> auth_servers;   // live servers: their parameters and phase-1 state are zeroed at shutdown
+  bftq::k9::AuthGroup* d_auth_group = nullptr;   // K9's group constants (public), built on first use
 };
 void priv_release(bftq_keyring* kr);             // decrypt_host.inc: zero and free a keyring's private-key table
 void keyring_detach(bftq_keyring* kr);           // a keyring that outlives its engine becomes parse-only
 void thrsa_shutdown(bftq_engine* e);             // thrsa_host.inc: zero and free every live share's fragments
 void thdsa_shutdown(bftq_engine* e);             // thdsa_host.inc: zero and free every live share's Y and (k, c) table
+void auth_shutdown(bftq_engine* e);              // auth_host.inc: zero and free every live server's allocation
 
 namespace {
 
@@ -697,6 +702,7 @@ void bftq_shutdown(bftq_engine* e) {
   }
   thrsa_shutdown(e);
   thdsa_shutdown(e);
+  auth_shutdown(e);
   for (auto& kv : e->host_allocs) cudaFreeHost(kv.first);
   for (auto* s : e->slots) {
     if (s->stream) { cudaStreamSynchronize(s->stream); cudaStreamDestroy(s->stream); }
@@ -1714,6 +1720,7 @@ int bftq_pgp_digest_batch(bftq_engine* e, const uint8_t* data_blob, const uint64
 #include "decrypt_host.inc"
 #include "thrsa_host.inc"
 #include "thdsa_host.inc"
+#include "auth_host.inc"
 
 // ---- quorum-descriptor builder ------------------------------------------------------------------
 // The descriptor the reference recomputes on EVERY call (client.go:64,101,141,238; server.go:182,211,237,300,473) is a

@@ -355,6 +355,34 @@ class Engine:
                                                    _ptr(nblob), _ptr(noff), _ptr(has), n, _ptr(err), _ptr(out), cap, _ptr(out_off)))
         return err[:n], [bytes(out[out_off[i]:out_off[i + 1]]) for i in range(n)]
 
+    def auth_server_create(self, params: bytes, proof: bytes):
+        """Registers one password-authentication server (auth.NewServer(params, proof)) on the device; returns its handle."""
+        h = C.c_void_p()
+        pb = np.frombuffer(params, np.uint8) if params else np.zeros(1, np.uint8)
+        fb = np.frombuffer(proof, np.uint8) if proof else np.zeros(1, np.uint8)
+        _lib.check(self._lib.bftq_auth_server_create(self._h, _ptr(pb), len(params), _ptr(fb), len(proof), C.byref(h)))
+        return h
+
+    def auth_server_destroy(self, server):
+        self._lib.bftq_auth_server_destroy(server)
+
+    def auth_server_respond_batch(self, servers, server_idx, phases, requests, rands):
+        """AuthServer.MakeResponse(phases[i], requests[i]) on servers[server_idx[i]], one call; rands[i]: b (256 bytes,
+        phase 1), the GCM nonce (12 bytes, phase 2), else b"".  (out_err int32[n], [answers])."""
+        n = len(requests)
+        blob, off = self._blob(list(requests))
+        rblob, roff = self._blob(list(rands))
+        tab = (C.c_void_p * max(1, len(servers)))(*[s.value for s in servers])
+        idx = np.ascontiguousarray(server_idx, np.uint32) if n else np.zeros(1, np.uint32)
+        ph = np.ascontiguousarray(phases, np.int32) if n else np.zeros(1, np.int32)
+        cap = sum(int(self._lib.bftq_auth_server_out_bound(servers[i], int(p))) for i, p in zip(server_idx, phases))
+        out = np.zeros(max(1, cap), np.uint8)
+        out_off = np.zeros(n + 1, np.uint64)
+        err = np.zeros(max(1, n), np.int32)
+        _lib.check(self._lib.bftq_auth_server_respond_batch(self._h, tab, len(servers), _ptr(idx), _ptr(ph), _ptr(blob), _ptr(off),
+                                                            _ptr(rblob), _ptr(roff), n, _ptr(err), _ptr(out), cap, _ptr(out_off)))
+        return err[:n], [bytes(out[out_off[i]:out_off[i + 1]]) for i in range(n)]
+
     def lagrange_exp_product_batch(self, p: int, q: int, x, ys):
         """auth.calculateSharedSecret: prod_j ys[i][j]^lambda_j mod p.  x: (B,k) ints, ys: B lists of k ints."""
         plen, qlen = (p.bit_length() + 7) // 8, (q.bit_length() + 7) // 8

@@ -50,6 +50,7 @@ extern "C" {
 #define BFTQ_ERR_INVALID_INPUT   -13   /* crypto.ErrInvalidInput (threshold RSA: the hash info leaves less than 3 padding bytes) */
 #define BFTQ_ERR_SHARE_NOT_FOUND -14   /* crypto.ErrShareNotFound (threshold DSA: no joint share for this node, or a stale nonce) */
 #define BFTQ_ERR_KEY_NOT_FOUND   -15   /* crypto.ErrKeyNotFound (threshold DSA: phase 3 without a phase 2 for the peer) */
+#define BFTQ_ERR_AUTH_FAILURE    -16   /* bftkv.ErrAuthenticationFailure (password authentication: Ni does not match) */
 
 /* ---- per-item status bytes (SURVEY §8b "Errors") --------------------------------------------
  * The reference collapses every failure to ErrInvalidSignature (crypto_pgp.go:325-327); the shim
@@ -614,6 +615,41 @@ int bftq_read_encrypted_responses_batch(bftq_keyring* kr, const bftq_qc_ids_t* q
                                         uint8_t* out_status, uint64_t* out_ts, uint32_t* out_value_off, uint32_t* out_value_len,
                                         uint8_t* out_plain_blob, uint32_t* out_plain_len,
                                         uint8_t* out_decision, uint32_t* out_winner, uint32_t* out_decided_at);
+
+/* ---- threshold password authentication, server half (crypto/auth/auth.go:168-237, K9) ---------------------------
+ * bftq_auth_server_create is NewServer(params, proof): params as serializeParams writes them (int32 x, then chunks y, v
+ * and salt, each a u64 big-endian length and its bytes).  y, v, the salt's HMAC key block and the proof go to one device
+ * allocation per server, zeroed before it is freed (bftq_auth_server_destroy, bftq_shutdown); the host copies of y and v
+ * are wiped.  Returns
+ *   BFTQ_ERR_MALFORMED        truncated framing
+ *   BFTQ_ERR_UNSUPPORTED_KEY  y or v longer than 256 bytes (setAuth stores params unverified: keep that session on Go)
+ * No secret reaches an error text or the statistics. */
+typedef struct bftq_auth_server bftq_auth_server;
+int bftq_auth_server_create(bftq_engine* e, const uint8_t* params, uint64_t params_len, const uint8_t* proof, uint64_t proof_len,
+                            bftq_auth_server** out);
+void bftq_auth_server_destroy(bftq_auth_server* s);
+/* The largest answer of one item: phase 0: 4 + 8 + 256 + 8 + |salt|; phase 1: 8 + 256; phase 2: 8 + |proof| + 16 + 8 + 12;
+ * any other phase: 0. */
+uint64_t bftq_auth_server_out_bound(const bftq_auth_server* s, int32_t phase);
+/* One scheduling tick of MakeResponse(phase[i], req[i]) on handles[handle_idx[i]], phases mixed.  req: the adata as
+ * received (X, Xi or Ni); rand: the randomness Go drew (phase 1: b, exactly 256 big-endian bytes; phase 2: the 12-byte
+ * GCM nonce; ignored otherwise).  A wrong rand length, a server listed twice, or out_cap below the sum of
+ * bftq_auth_server_out_bound(server, phase) over the items is BFTQ_ERR_INVALID_ARG before any work.
+ *   phase 0  out = int32 x | chunk(Yi.Bytes()) | chunk(salt), Yi = X^y mod p
+ *   phase 1  out = chunk(Bi.Bytes()), Bi = v^b mod p; stores keySched(Ki.Bytes(), salt)'s ke and the MAC
+ *            HMAC-SHA256(km, Xi || Bi.Bytes()) on the device (Ki = Xi^b mod p); a repeated phase 1 overwrites them
+ *   phase 2  out = chunk(AES-128-GCM(ke).Seal(nonce, proof, mac) || tag) | chunk(nonce) when Ni equals the MAC (constant
+ *            time), else out_err[i] = BFTQ_ERR_AUTH_FAILURE.  Either way the server's phase-1 state is zeroed.
+ *            Divergence: a server with no phase-1 state fails here.  The reference compares Ni against a nil MAC, so
+ *            an empty Ni passes and the proof is sealed under an all-zero key.
+ *   other    empty answer, out_err[i] = 0, no state change.
+ * out_off[i] .. out_off[i+1]: item i's answer in out_blob.  Per-call device and host buffers that held b or Ki are
+ * zeroed before the call returns.  The attempts counter, its delay and ErrAuthTooManyAttempts, request framing and the
+ * per-variable session map stay in Go (INTEGRATION.md). */
+int bftq_auth_server_respond_batch(bftq_engine* e, bftq_auth_server* const* handles, uint32_t n_handles, const uint32_t* handle_idx,
+                                   const int32_t* phase, const uint8_t* req_blob, const uint64_t* req_off, const uint8_t* rand_blob,
+                                   const uint64_t* rand_off, uint64_t n_items, int32_t* out_err, uint8_t* out_blob, uint64_t out_cap,
+                                   uint64_t* out_off);
 
 /* ---- quorum-descriptor builder (host only; no GPU needed) --------------------------------------
  * The step before the tally: wotqs.ChooseQuorum over the PGP trust graph
