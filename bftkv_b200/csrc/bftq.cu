@@ -20,6 +20,8 @@
 #include "pgp_host.hpp"
 #include "wotqs_host.hpp"
 #include "bignum_host.hpp"
+#include "device_secret.hpp"
+#include "wire_host.hpp"
 
 #include <algorithm>
 #include <array>
@@ -215,24 +217,29 @@ struct bftq_engine {
   cpu_set_t numa_cpus;
   std::map<void*, size_t> host_allocs;           // bftq_host_alloc blocks
   uint32_t packer_flags = 0;   // BFTQ_F_* the packet-level entry points pass to K1 (bftq_engine_set_verify_flags / env BFTQ_STRICT_RANGE)
-  std::mutex kr_mu;
-  std::vector<bftq_keyring*> keyrings;           // live keyrings: their private-key tables are zeroed at shutdown
-  std::mutex thrsa_mu;
-  std::vector<bftq_thrsa_share*> thrsa_shares;   // live threshold-RSA shares: their fragments are zeroed at shutdown
-  std::mutex thdsa_mu;                           // threshold-DSA shares and their (k, c) tables
-  std::vector<bftq_thdsa_share*> thdsa_shares;   // live threshold-DSA shares: Y and the tables are zeroed at shutdown
+  // live handles that hold key material on the device, zeroed and freed at shutdown
+  HandleList<bftq_keyring> keyrings;             // private-key tables
+  HandleList<bftq_thrsa_share> thrsa;            // threshold-RSA fragments
+  HandleList<bftq_thdsa_share> thdsa;            // threshold-DSA Y and (k, c) tables; mu also covers the sign calls
+  HandleList<bftq_auth_server> auth;             // auth parameters and phase-1 state; mu also covers the respond calls
   uint32_t* d_p256_base = nullptr;               // K8's fixed-base table of P-256 (public), built on first use
-  std::mutex auth_mu;                            // password-authentication servers and the calls that use them
-  std::vector<bftq_auth_server*> auth_servers;   // live servers: their parameters and phase-1 state are zeroed at shutdown
   bftq::k9::AuthGroup* d_auth_group = nullptr;   // K9's group constants (public), built on first use
 };
-void priv_release(bftq_keyring* kr);             // decrypt_host.inc: zero and free a keyring's private-key table
-void keyring_detach(bftq_keyring* kr);           // a keyring that outlives its engine becomes parse-only
-void thrsa_shutdown(bftq_engine* e);             // thrsa_host.inc: zero and free every live share's fragments
-void thdsa_shutdown(bftq_engine* e);             // thdsa_host.inc: zero and free every live share's Y and (k, c) table
-void auth_shutdown(bftq_engine* e);              // auth_host.inc: zero and free every live server's allocation
 
 namespace {
+
+// Blocks for n items at B / 4 items per block (four lanes per item), at most `cap` per SM: the kernel strides over the rest.
+unsigned capped_grid(const bftq_engine* e, uint64_t n, int B, uint64_t cap) {
+  return (unsigned)std::min<uint64_t>((n + B / 4 - 1) / (B / 4), (uint64_t)std::max(1, e->sm_count) * cap);
+}
+// One of the engine's lazily built public tables (freed at shutdown); nothing stays allocated when the upload fails.
+template <class T> int upload_table(const T* host, size_t count, T** out, const char* what) {
+  T* d = nullptr;
+  if (cudaMalloc(&d, count * sizeof(T)) != cudaSuccess) { cudaGetLastError(); return fail(BFTQ_ERR_NOMEM, std::string(what) + ": device allocation failed"); }
+  if (cudaMemcpy(d, host, count * sizeof(T), cudaMemcpyHostToDevice) != cudaSuccess) { cudaFree(d); return fail(BFTQ_ERR_CUDA, std::string(what) + " upload failed"); }
+  *out = d;
+  return BFTQ_OK;
+}
 
 // A device block of at least `bytes` (the smallest cached one that fits, else a fresh cudaMalloc).  The caller must have
 // finished every stream that touched the block before releasing it.
@@ -690,37 +697,6 @@ int bftq_bind_thread(bftq_engine* e) {
   if (!e) return fail(BFTQ_ERR_INVALID_ARG, "NULL argument");
   numa_bind_this_thread(e);
   return e->numa_valid ? e->numa_node : -1;
-}
-
-void bftq_shutdown(bftq_engine* e) {
-  if (!e) return;
-  cudaSetDevice(e->device);
-  {
-    std::lock_guard<std::mutex> g(e->kr_mu);
-    for (bftq_keyring* kr : e->keyrings) { priv_release(kr); keyring_detach(kr); }
-    e->keyrings.clear();
-  }
-  thrsa_shutdown(e);
-  thdsa_shutdown(e);
-  auth_shutdown(e);
-  for (auto& kv : e->host_allocs) cudaFreeHost(kv.first);
-  for (auto* s : e->slots) {
-    if (s->stream) { cudaStreamSynchronize(s->stream); cudaStreamDestroy(s->stream); }
-    if (s->done) cudaEventDestroy(s->done);
-    if (s->h_pinned) cudaFreeHost(s->h_pinned);
-    if (s->d_buf) cudaFree(s->d_buf);
-    delete s;
-  }
-  if (e->d_keys) cudaFree(e->d_keys);
-  if (e->d_keys32) cudaFree(e->d_keys32);
-  cudaDeviceSynchronize();
-  for (auto& b : e->scratch.free_list) cudaFree(b.first);
-  for (cudaEvent_t ev : e->ed.pending) cudaEventDestroy(ev);
-  if (e->ed.d_tab) cudaFree(e->ed.d_tab);
-  if (e->ed.d_tabB) cudaFree(e->ed.d_tabB);
-  if (e->ed.d_hdr) cudaFree(e->ed.d_hdr);
-  for (void* p : e->retired) cudaFree(p);
-  delete e;
 }
 
 int bftq_device_sm_count(bftq_engine* e) { return e ? e->sm_count : BFTQ_ERR_INVALID_ARG; }
@@ -1721,6 +1697,38 @@ int bftq_pgp_digest_batch(bftq_engine* e, const uint8_t* data_blob, const uint64
 #include "thrsa_host.inc"
 #include "thdsa_host.inc"
 #include "auth_host.inc"
+
+extern "C" {
+// After the .inc files: the handle lists detach handle types defined there.
+void bftq_shutdown(bftq_engine* e) {
+  if (!e) return;
+  cudaSetDevice(e->device);
+  e->keyrings.shutdown();
+  e->thrsa.shutdown();
+  e->thdsa.shutdown();
+  e->auth.shutdown();
+  for (auto& kv : e->host_allocs) cudaFreeHost(kv.first);
+  for (auto* s : e->slots) {
+    if (s->stream) { cudaStreamSynchronize(s->stream); cudaStreamDestroy(s->stream); }
+    if (s->done) cudaEventDestroy(s->done);
+    if (s->h_pinned) cudaFreeHost(s->h_pinned);
+    if (s->d_buf) cudaFree(s->d_buf);
+    delete s;
+  }
+  if (e->d_keys) cudaFree(e->d_keys);
+  if (e->d_keys32) cudaFree(e->d_keys32);
+  if (e->d_p256_base) cudaFree(e->d_p256_base);
+  if (e->d_auth_group) cudaFree(e->d_auth_group);
+  cudaDeviceSynchronize();
+  for (auto& b : e->scratch.free_list) cudaFree(b.first);
+  for (cudaEvent_t ev : e->ed.pending) cudaEventDestroy(ev);
+  if (e->ed.d_tab) cudaFree(e->ed.d_tab);
+  if (e->ed.d_tabB) cudaFree(e->ed.d_tabB);
+  if (e->ed.d_hdr) cudaFree(e->ed.d_hdr);
+  for (void* p : e->retired) cudaFree(p);
+  delete e;
+}
+}  // extern "C"
 
 // ---- quorum-descriptor builder ------------------------------------------------------------------
 // The descriptor the reference recomputes on EVERY call (client.go:64,101,141,238; server.go:182,211,237,300,473) is a
