@@ -222,23 +222,20 @@ pgp_digest_kernel(const uint8_t* __restrict__ data_blob, const uint64_t* __restr
   }
 }
 
-inline bool digest_on_device(uint32_t hash_alg) { return hash_alg == 1 || hash_alg == 2 || hash_alg == 8 || hash_alg == 9 || hash_alg == 10 || hash_alg == 11; }
-
-inline cudaError_t launch_pgp_digest(uint32_t hash_alg, const uint8_t* data_blob, const uint64_t* data_off, const uint32_t* data_idx,
-                                     const uint8_t* suffix_blob, const uint64_t* suffix_off, uint64_t n, uint8_t* out, const uint16_t* tags,
-                                     uint8_t* pre, cudaStream_t st) {
-  const int block = 128;
-  const unsigned grid = (unsigned)((n + block - 1) / block);
+using PgpDigestKernel = void (*)(const uint8_t*, const uint64_t*, const uint32_t*, const uint8_t*, const uint64_t*, uint64_t, uint8_t*,
+                                 const uint16_t*, uint8_t*);
+// The digest kernel of an OpenPGP hash id, or null when the device does not compute that digest.
+inline PgpDigestKernel pgp_digest_kernel_for(uint32_t hash_alg) {
   switch (hash_alg) {
-    case 1: pgp_digest_kernel<1><<<grid, block, 0, st>>>(data_blob, data_off, data_idx, suffix_blob, suffix_off, n, out, tags, pre); break;
-    case 2: pgp_digest_kernel<2><<<grid, block, 0, st>>>(data_blob, data_off, data_idx, suffix_blob, suffix_off, n, out, tags, pre); break;
-    case 8: pgp_digest_kernel<8><<<grid, block, 0, st>>>(data_blob, data_off, data_idx, suffix_blob, suffix_off, n, out, tags, pre); break;
-    case 9: pgp_digest_kernel<9><<<grid, block, 0, st>>>(data_blob, data_off, data_idx, suffix_blob, suffix_off, n, out, tags, pre); break;
-    case 10: pgp_digest_kernel<10><<<grid, block, 0, st>>>(data_blob, data_off, data_idx, suffix_blob, suffix_off, n, out, tags, pre); break;
-    case 11: pgp_digest_kernel<11><<<grid, block, 0, st>>>(data_blob, data_off, data_idx, suffix_blob, suffix_off, n, out, tags, pre); break;
-    default: return cudaErrorInvalidValue;
+    case 1: return pgp_digest_kernel<1>;
+    case 2: return pgp_digest_kernel<2>;
+    case 8: return pgp_digest_kernel<8>;
+    case 9: return pgp_digest_kernel<9>;
+    case 10: return pgp_digest_kernel<10>;
+    case 11: return pgp_digest_kernel<11>;
+    default: return nullptr;
   }
-  return cudaGetLastError();
 }
+inline bool digest_on_device(uint32_t hash_alg) { return pgp_digest_kernel_for(hash_alg) != nullptr; }
 
 }  // namespace bftq

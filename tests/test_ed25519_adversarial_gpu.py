@@ -83,7 +83,7 @@ def test_table_path_every_row(vec):
     with _engine(True) as eng:
         got, dl = _run(eng, vec, idx)
         _check(got, vec, idx)
-        assert dl == 4                                   # table builds (base point + keys) + accumulate + finish
+        assert dl == 6                                   # base-point table 2, key tables 2, accumulate and finish 2
         got, dl = _run(eng, vec, idx)
         _check(got, vec, idx)
         assert dl == 2                                   # every key cached: accumulate + finish only
@@ -167,7 +167,7 @@ def test_two_encodings_of_one_point_are_two_slots(vec):
         idx = _replicated(vec, sel_c)
         got, dl = _run(eng, vec, idx)
         _check(got, vec, idx)
-        assert dl == 4
+        assert dl == 6                                   # base-point table 2, key tables 2, accumulate and finish 2
         idx = _replicated(vec, sel_c + sel_o, seed=3)
         got, dl = _run(eng, vec, idx)
         _check(got, vec, idx)

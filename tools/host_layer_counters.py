@@ -1,8 +1,9 @@
 """What the batched host entry points did and returned on seeded inputs: python tools/host_layer_counters.py [out.json]
 
 Calls bftq_rsa_verify_batch (40 000 items), bftq_verify_read_batch, bftq_signature_verify_batch (with items the GPU parser
-flags), bftq_collective_verify_batch and bftq_read_responses_batch, and after each prints the bftq_stats counters that depend
-on the host layer's plumbing only (launches, items, bytes copied, chunks, GPU-/host-parsed messages) and a SHA-256 of every
+flags), bftq_collective_verify_batch, bftq_read_responses_batch, bftq_message_decrypt_batch,
+bftq_read_encrypted_responses_batch and one small call of every flat entry point tests/test_launch_accounting_gpu.py pins,
+and after each prints the bftq_stats counters that depend on the host layer's plumbing only (launches, items, bytes copied, chunks, GPU-/host-parsed messages) and a SHA-256 of every
 output array.  A change to the host layer that is meant to keep behaviour is run against both builds (BFTQ_LIB_PATH selects
 the library) and the two outputs are compared: they must be equal.  BFTQ_HOST_THREADS=1 makes the chunk counts deterministic."""
 import hashlib
@@ -12,11 +13,13 @@ import random
 import sys
 
 os.environ["BFTQ_HOST_THREADS"] = "1"
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
 import numpy as np  # noqa: E402
 
 from bftkv_b200 import Engine, workload  # noqa: E402
-from bftkv_b200.crypto_gpu import CollectiveSignature, Keyring, Quorum, Signature, read_responses_batch  # noqa: E402
+from bftkv_b200.crypto_gpu import CollectiveSignature, Keyring, Message, Quorum, Signature, read_encrypted_responses_batch, read_responses_batch  # noqa: E402
+from test_launch_accounting_gpu import flat_calls  # noqa: E402
 
 COUNTERS = ("launches", "items", "h2d_bytes", "d2h_bytes", "packer_chunks", "msg_gpu_items", "msg_host_items")
 
@@ -24,6 +27,8 @@ COUNTERS = ("launches", "items", "h2d_bytes", "d2h_bytes", "packer_chunks", "msg
 def digest(x):
     if isinstance(x, np.ndarray):
         return hashlib.sha256(np.ascontiguousarray(x).tobytes()).hexdigest()
+    if isinstance(x, (tuple, list)):
+        return hashlib.sha256("".join(digest(v) for v in x).encode()).hexdigest()
     return hashlib.sha256(repr(x).encode()).hexdigest()
 
 
@@ -38,10 +43,11 @@ def main():
     report = {}
     eng = Engine(0)
 
-    def step(name, fn):
-        s0 = eng.stats()
+    def step(name, fn, e=eng):
+        s0 = e.stats()
         out = fn()
-        s1 = eng.stats()
+        s1 = e.stats()
+        out = out if isinstance(out, dict) else {"out": out}
         report[name] = {"stats": {k: s1[k] - s0[k] for k in COUNTERS}, "outputs": {k: digest(v) for k, v in out.items()}}
         print(name, json.dumps(report[name]), flush=True)
 
@@ -88,7 +94,24 @@ def main():
     kr2.register(ra["keyring"])
     step("read_responses_batch", lambda: read_responses_batch(kr2, [(5, 16, 6, 11, ra["ids"])], ra["op_off"], ra["peer_ids"], ra["msgs"],
                                                              ra["nonces"], pre_status=ra["pre_status"]))
+    # ---- the decryption layer: the same answers encrypted to a client key
+    ck = workload.load_keys(17)[16]
+    cblock, cid = workload.pgp_public_key_block(ck, workload._private_key(ck), b"client <client@bftq.test>")
+    raws, _ = workload.encrypt_answers(ra["msgs"], ck, cid)
+    kr2.register(cblock, priv=True)
+    assert kr2.register_private(workload.secret_key_packet(ck)) == 1
+    step("message_decrypt_batch", lambda: Message(kr2).decrypt_batch(raws[:512]))
+    step("read_encrypted_responses_batch", lambda: read_encrypted_responses_batch(kr2, [(5, 16, 6, 11, ra["ids"])], ra["op_off"], ra["peer_ids"],
+                                                                                 raws, ra["nonces"], pre_status=ra["pre_status"]))
     kr2.close()
+
+    # ---- one small call of every flat entry point (the Ed25519 calls expect an engine whose table cache is empty)
+    fresh = Engine(0)
+    q = fresh.quorum_create([(1, 4, 2, 3, [0, 1, 2, 3])])
+    for name, call in flat_calls(fresh, q):
+        step(name, call, fresh)
+    fresh.quorum_destroy(q)
+    fresh.close()
     eng.close()
     if len(sys.argv) > 1:
         with open(sys.argv[1], "w") as f:
