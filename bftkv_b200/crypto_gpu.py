@@ -582,3 +582,94 @@ class AuthServer:
         if self._h is not None:
             self.engine.auth_server_destroy(self._h)
             self._h = None
+
+
+ErrNoAuthenticationData = "crypto: no authentication data"
+ErrInsufficientNumberOfSecrets = "crypto: insufficient number of secrets"
+AUTH_Q = (AUTH_P - 1) // 2
+AUTH_INITIATE, AUTH_CIPHER_KEY = -1, -2
+_AUTH_CLIENT_ERRORS = {-8: "malformed answer", -17: ErrNoAuthenticationData, -18: ErrDecryptionFailed, -19: ErrInsufficientNumberOfSecrets}
+
+
+class AuthClient:
+    """The client half of crypto/auth: NewClient / Initiate / ProcessResponse / Done / GetCipherKey over a session
+    registered on the device.  The password, a, a' and gs stay on the device.  `rand(n)` draws an integer below n (default
+    secrets.randbelow, injectable for tests): a = rand(q) at Initiate, and a' = rand(q) per secret when a phase-0 answer
+    completes the set, in the order the secrets first arrived.  Maps are dicts in that order; None is Go's nil map."""
+
+    def __init__(self, engine: Engine, password: bytes, n: int, k: int, rand=None):
+        import secrets
+        self.engine = engine
+        self.n, self.k = n, k
+        self._rand = rand if rand is not None else secrets.randbelow
+        self._peers = []                        # distinct phase-0 peers so far: how many a' a completing answer needs
+        self._h = engine.auth_client_create(password, n, k)
+
+    def _rand_for(self, op: int, peer_id: int) -> bytes:
+        if op == AUTH_INITIATE:
+            return self._rand(AUTH_Q).to_bytes(256, "big")
+        if op == 0:
+            m = len(self._peers) + (peer_id not in self._peers)
+            if m >= self.k:
+                return b"".join(self._rand(AUTH_Q).to_bytes(256, "big") for _ in range(m))
+        return b""
+
+    @staticmethod
+    def _parse_map(b: bytes) -> dict:
+        import struct
+        cnt, pos, out = struct.unpack(">I", b[:4])[0], 4, {}
+        for _ in range(cnt):
+            pid, ln = struct.unpack(">QQ", b[pos:pos + 16])
+            out[pid] = b[pos + 16:pos + 16 + ln]
+            pos += 16 + ln
+        return out
+
+    @classmethod
+    def process_batch(cls, engine: Engine, clients: Sequence["AuthClient"], ops: Sequence[int], datas: Sequence[bytes],
+                      peer_ids: Sequence[int], rands: Optional[Sequence[bytes]] = None):
+        """Items (clients[i], ops[i], datas[i], peer_ids[i]) in one call, applied as if one at a time in order:
+        [(result, err)].  Initiate's result is X, a phase's the returned map (or None), GetCipherKey's the 32-byte key.
+        rands: the randomness per item (None: drawn here)."""
+        tab = list({id(c): c for c in clients}.values())
+        pos = {id(c): j for j, c in enumerate(tab)}
+        if rands is None:
+            rands = []
+            for c, op, pid in zip(clients, ops, peer_ids):
+                rands.append(c._rand_for(op, pid))
+                if op == 0 and pid not in c._peers:
+                    c._peers.append(pid)
+        err, has, outs = engine.auth_client_process_batch([c._h for c in tab], [pos[id(c)] for c in clients], list(ops), list(peer_ids),
+                                                          list(datas), list(rands))
+        res = []
+        for c, op, pid, e, hm, o in zip(clients, ops, peer_ids, err, has, outs):
+            if op == 0 and e == 0 and pid not in c._peers:
+                c._peers.append(pid)
+            if e != 0:
+                res.append((None, _AUTH_CLIENT_ERRORS.get(int(e), int(e))))
+            elif op in (AUTH_INITIATE, AUTH_CIPHER_KEY):
+                res.append((o, None))
+            else:
+                res.append((cls._parse_map(o) if hm else None, None))
+        return res
+
+    def initiate(self, nodes: Sequence[int]) -> dict:
+        """Initiate(nodes): {node id: X}."""
+        X, _ = self.process_batch(self.engine, [self], [AUTH_INITIATE], [b""], [0])[0]
+        return {nid: X for nid in nodes}
+
+    def process_response(self, phase: int, data: bytes, peer_id: int):
+        """ProcessResponse(phase, data, peer): (map or None, err)."""
+        return self.process_batch(self.engine, [self], [phase], [data], [peer_id])[0]
+
+    @staticmethod
+    def done(phase: int) -> bool:
+        return phase > 2
+
+    def get_cipher_key(self):
+        """GetCipherKey(): (key, err)."""
+        return self.process_batch(self.engine, [self], [AUTH_CIPHER_KEY], [b""], [0])[0]
+
+    def close(self):
+        if self._h is not None:
+            self.engine.auth_client_destroy(self._h)
+            self._h = None

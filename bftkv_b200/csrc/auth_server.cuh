@@ -5,7 +5,8 @@
 //                          phase 1's Bi = v^b and Ki = Xi^b.  One 4-lane group per item, r32::ct_window_pow.
 //   auth_kdf_mac_kernel    phase 1: keySched (HKDF-SHA256, salt as the extract key, Ki.Bytes() as the input key material,
 //                          nil info; km = OKM[0:16], ke = OKM[16:32]) and the MAC HMAC-SHA256(km, Xi || Bi.Bytes()).
-//                          One thread per item; writes ke and the MAC into the server's allocation.
+//                          One thread per item; writes ke and the MAC where the item says: the server's allocation, or
+//                          for the client half (auth_client.cuh) the session's slot and the per-call buffer.
 //   auth_gcm_seal_kernel   phase 2: the MAC check (constant time) and AES-128-GCM(ke).Seal(nonce, proof, aad = mac).
 //                          One thread per item; wipes the server's phase-1 state whatever the outcome.
 //
@@ -23,7 +24,7 @@
 // existing decrypt path.
 // No K9 kernel uses local memory (tests/test_auth_host.py checks the SASS).
 //
-// The HMAC / HKDF and GHASH cores are __host__ __device__: tests/harness/auth_host.cpp builds them with g++.
+// The HMAC / HKDF, GHASH and GCM cores are __host__ __device__: tests/harness/auth_host.cpp builds them with g++.
 #pragma once
 #include <cstdint>
 #include "sha256.cuh"
@@ -152,6 +153,65 @@ BFTQ_SHA_HD_FI void gf128_mul(uint64_t& xh, uint64_t& xl, const uint64_t hh, con
   xh = zh; xl = zl;
 }
 
+BFTQ_SHA_HD_FI void gcm_block(uint64_t& xh, uint64_t& xl, const uint32_t s0, const uint32_t s1, const uint32_t s2, const uint32_t s3,
+                              const uint64_t hh, const uint64_t hl) {
+  xh ^= ((uint64_t)s0 << 32) | s1;
+  xl ^= ((uint64_t)s2 << 32) | s3;
+  gf128_mul(xh, xl, hh, hl);
+}
+
+// Big-endian word j of the 16-byte block `blk` of p (len bytes), zero past the end.
+BFTQ_SHA_HD_FI uint32_t gcm_word(const uint8_t* p, const uint64_t len, const uint64_t blk, const int j) {
+  uint32_t v = 0;
+  for (int b = 0; b < 4; b++) {
+    const uint64_t pos = blk * 16 + 4 * j + b;
+    v = (v << 8) | (pos < len ? (uint32_t)p[pos] : 0u);
+  }
+  return v;
+}
+
+// AES-GCM with a 12-byte nonce (n0, n1, n2: its big-endian words; NIST SP 800-38D): H = E(0), J0 = nonce || 1, block b of
+// src (len bytes) is xored with E(inc32(J0) + b).  dst (nullable) receives src xor the key stream.  GHASH runs over aad
+// (aad_len bytes) and the ciphertext, which is what dst receives when `seal`, else src; tag = GHASH xor E(J0).
+// enc(s0, s1, s2, s3) encrypts one block in place under the key.  Trip counts depend on aad_len and len only.
+template <class Enc>
+BFTQ_SHA_HD_FI void gcm_core(const Enc& enc, const uint32_t n0, const uint32_t n1, const uint32_t n2, const uint8_t* aad, const uint64_t aad_len,
+                             const uint8_t* src, const uint64_t len, uint8_t* dst, const bool seal, uint8_t (&tag)[16]) {
+  uint32_t h0 = 0u, h1 = 0u, h2 = 0u, h3 = 0u;
+  enc(h0, h1, h2, h3);
+  const uint64_t hh = ((uint64_t)h0 << 32) | h1, hl = ((uint64_t)h2 << 32) | h3;
+  uint64_t xh = 0, xl = 0;
+#pragma unroll 1
+  for (uint64_t blk = 0; blk * 16 < aad_len; blk++)
+    gcm_block(xh, xl, gcm_word(aad, aad_len, blk, 0), gcm_word(aad, aad_len, blk, 1), gcm_word(aad, aad_len, blk, 2), gcm_word(aad, aad_len, blk, 3), hh, hl);
+#pragma unroll 1
+  for (uint64_t blk = 0; blk * 16 < len; blk++) {
+    uint32_t k[4] = {n0, n1, n2, (uint32_t)(blk + 2)};                   // inc32(J0) + blk
+    enc(k[0], k[1], k[2], k[3]);
+    uint32_t c[4];
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+      uint32_t v = 0;
+#pragma unroll
+      for (int b = 0; b < 4; b++) {
+        const uint64_t pos = blk * 16 + 4 * j + b;
+        const uint32_t in = pos < len ? (uint32_t)src[pos] : 0u;
+        const uint32_t by = pos < len ? (in ^ (uint8_t)(k[j] >> (24 - 8 * b))) : 0u;
+        if (dst && pos < len) dst[pos] = (uint8_t)by;
+        v = (v << 8) | (seal ? by : in);
+      }
+      c[j] = v;
+    }
+    gcm_block(xh, xl, c[0], c[1], c[2], c[3], hh, hl);
+  }
+  gcm_block(xh, xl, (uint32_t)((aad_len * 8) >> 32), (uint32_t)(aad_len * 8), (uint32_t)((len * 8) >> 32), (uint32_t)(len * 8), hh, hl);
+  uint32_t s0 = n0, s1 = n1, s2 = n2, s3 = 1u;                               // J0
+  enc(s0, s1, s2, s3);
+  const uint64_t th = xh ^ (((uint64_t)s0 << 32) | s1), tl = xl ^ (((uint64_t)s2 << 32) | s3);
+#pragma unroll
+  for (int b = 0; b < 8; b++) { tag[b] = (uint8_t)(th >> (56 - 8 * b)); tag[8 + b] = (uint8_t)(tl >> (56 - 8 * b)); }
+}
+
 #ifdef __CUDACC__
 using r32::T;
 using k6::K6B_BLOCK;
@@ -231,8 +291,10 @@ auth_pow_kernel(const AuthGroup* __restrict__ G, const PowItem* __restrict__ ite
   }
 }
 
-// Phase 1's keys and MAC.  Ki and Bi are rows of auth_pow_kernel's output.
-struct KdfItem { uint64_t state; uint64_t xi; uint32_t xi_len, ki_row, bi_row, pad; };
+// Phase 1's keys and MAC.  Ki is a row of auth_pow_kernel's output; Bi is that too (bi == 0: row bi_row, the server's own
+// Bi) or bi_len bytes at bi (the client's, as received).  salt_key: the salt's HMAC key block; ke (16 bytes), mac (32
+// bytes) and flag (set to 1) are where the results go.
+struct KdfItem { uint64_t salt_key, ke, mac, flag, xi, bi; uint32_t xi_len, bi_len, ki_row, bi_row; };
 
 struct KiBytes {
   const uint8_t* p;
@@ -245,35 +307,38 @@ auth_kdf_mac_kernel(const KdfItem* __restrict__ items, const uint64_t n_items, c
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_items) return;
   const KdfItem it = items[i];
-  AuthState* S = reinterpret_cast<AuthState*>(it.state);
+  const uint32_t* salt_key = reinterpret_cast<const uint32_t*>(it.salt_key);
+  uint8_t* ke = reinterpret_cast<uint8_t*>(it.ke);
+  uint8_t* mo = reinterpret_cast<uint8_t*>(it.mac);
   uint32_t sk[16], t[8], km[4], mac[8];
 #pragma unroll
-  for (int k = 0; k < 16; k++) sk[k] = S->salt_key[k];
-  const uint32_t kl = pow_len[it.ki_row], bl = pow_len[it.bi_row];
+  for (int k = 0; k < 16; k++) sk[k] = salt_key[k];
+  const uint32_t kl = pow_len[it.ki_row];
   hkdf_sha256_32(t, sk, KiBytes{pow_be + (uint64_t)it.ki_row * kAuthBytes + (kAuthBytes - kl)}, kl);
 #pragma unroll
   for (int k = 0; k < 4; k++) km[k] = t[k];
-  auth_mac(mac, km, reinterpret_cast<const uint8_t*>(it.xi), it.xi_len, pow_be + (uint64_t)it.bi_row * kAuthBytes + (kAuthBytes - bl), bl);
+  const uint32_t bl = it.bi ? it.bi_len : pow_len[it.bi_row];
+  const uint8_t* bi = it.bi ? reinterpret_cast<const uint8_t*>(it.bi) : pow_be + (uint64_t)it.bi_row * kAuthBytes + (kAuthBytes - bl);
+  auth_mac(mac, km, reinterpret_cast<const uint8_t*>(it.xi), it.xi_len, bi, bl);
 #pragma unroll
   for (int k = 0; k < 4; k++)
 #pragma unroll
-    for (int b = 0; b < 4; b++) S->ke[4 * k + b] = (uint8_t)(t[4 + k] >> (24 - 8 * b));
+    for (int b = 0; b < 4; b++) ke[4 * k + b] = (uint8_t)(t[4 + k] >> (24 - 8 * b));
 #pragma unroll
   for (int k = 0; k < 8; k++)
 #pragma unroll
-    for (int b = 0; b < 4; b++) S->mac[4 * k + b] = (uint8_t)(mac[k] >> (24 - 8 * b));
-  S->has_p1 = 1u;
+    for (int b = 0; b < 4; b++) mo[4 * k + b] = (uint8_t)(mac[k] >> (24 - 8 * b));
+  *reinterpret_cast<uint32_t*>(it.flag) = 1u;
 }
+
+// One AES-128 block under the key schedule rk (K6b's, S-box sb in shared memory): gcm_core's block cipher.
+struct AesEnc {
+  const uint32_t* rk; const uint8_t* sb;
+  __device__ __forceinline__ void operator()(uint32_t& s0, uint32_t& s1, uint32_t& s2, uint32_t& s3) const { aes_encrypt<4>(rk, s0, s1, s2, s3, sb); }
+};
 
 // Phase 2.  ni: the request (ni_len bytes), nonce: 12 bytes, out: proof_len + 16 bytes (ciphertext || tag).
 struct SealItem { uint64_t state; uint64_t ni; uint64_t nonce; uint64_t out; uint32_t ni_len, pad; };
-
-__device__ __forceinline__ void gcm_block(uint64_t& xh, uint64_t& xl, const uint32_t s0, const uint32_t s1, const uint32_t s2, const uint32_t s3,
-                                          const uint64_t hh, const uint64_t hl) {
-  xh ^= ((uint64_t)s0 << 32) | s1;
-  xl ^= ((uint64_t)s2 << 32) | s3;
-  gf128_mul(xh, xl, hh, hl);
-}
 
 // ok[i] = 1 when the item's MAC matched and out holds the sealed proof, 0 otherwise.
 __global__ void __launch_bounds__(K6B_BLOCK)
@@ -294,42 +359,13 @@ auth_gcm_seal_kernel(const SealItem* __restrict__ items, const uint64_t n_items,
     if (good) {
       aes_expand<4>(S->ke, rk, sb);
       const uint8_t* nn = reinterpret_cast<const uint8_t*>(it.nonce);
-      const uint32_t n0 = load_be32(nn, 0, 12), n1 = load_be32(nn, 4, 12), n2 = load_be32(nn, 8, 12);
-      uint32_t h0 = 0u, h1 = 0u, h2 = 0u, h3 = 0u;
-      aes_encrypt<4>(rk, h0, h1, h2, h3, sb);
-      const uint64_t hh = ((uint64_t)h0 << 32) | h1, hl = ((uint64_t)h2 << 32) | h3;
-      uint64_t xh = 0, xl = 0;
-      const uint8_t* mac = S->mac;
-      gcm_block(xh, xl, load_be32(mac, 0, 32), load_be32(mac, 4, 32), load_be32(mac, 8, 32), load_be32(mac, 12, 32), hh, hl);
-      gcm_block(xh, xl, load_be32(mac, 16, 32), load_be32(mac, 20, 32), load_be32(mac, 24, 32), load_be32(mac, 28, 32), hh, hl);
       const uint64_t len = S->proof_len;
       const uint8_t* pf = reinterpret_cast<const uint8_t*>(S) + sizeof(AuthState);
       uint8_t* out = reinterpret_cast<uint8_t*>(it.out);
-#pragma unroll 1
-      for (uint64_t blk = 0; blk * 16 < len; blk++) {
-        uint32_t k[4] = {n0, n1, n2, (uint32_t)(blk + 2)};                 // inc32(J0) + blk
-        aes_encrypt<4>(rk, k[0], k[1], k[2], k[3], sb);
-        uint32_t c[4];
+      uint8_t tag[16];
+      gcm_core(AesEnc{rk, sb}, load_be32(nn, 0, 12), load_be32(nn, 4, 12), load_be32(nn, 8, 12), S->mac, 32, pf, len, out, true, tag);
 #pragma unroll
-        for (int j = 0; j < 4; j++) {
-          uint32_t v = 0;
-#pragma unroll
-          for (int b = 0; b < 4; b++) {
-            const uint64_t pos = blk * 16 + 4 * j + b;
-            const uint32_t by = pos < len ? (uint32_t)(pf[pos] ^ (uint8_t)(k[j] >> (24 - 8 * b))) : 0u;
-            if (pos < len) out[pos] = (uint8_t)by;
-            v = (v << 8) | by;
-          }
-          c[j] = v;
-        }
-        gcm_block(xh, xl, c[0], c[1], c[2], c[3], hh, hl);
-      }
-      gcm_block(xh, xl, 0u, 32u * 8u, (uint32_t)((len * 8) >> 32), (uint32_t)(len * 8), hh, hl);
-      uint32_t s0 = n0, s1 = n1, s2 = n2, s3 = 1u;                           // J0
-      aes_encrypt<4>(rk, s0, s1, s2, s3, sb);
-      const uint64_t th = xh ^ (((uint64_t)s0 << 32) | s1), tl = xl ^ (((uint64_t)s2 << 32) | s3);
-#pragma unroll
-      for (int b = 0; b < 8; b++) { out[len + b] = (uint8_t)(th >> (56 - 8 * b)); out[len + 8 + b] = (uint8_t)(tl >> (56 - 8 * b)); }
+      for (int b = 0; b < 16; b++) out[len + b] = tag[b];
     }
     ok[i] = good ? 1 : 0;
 #pragma unroll

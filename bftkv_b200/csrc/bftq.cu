@@ -17,6 +17,7 @@
 #include "thrsa_sign.cuh"
 #include "thdsa_sign.cuh"
 #include "auth_server.cuh"
+#include "auth_client.cuh"
 #include "pgp_host.hpp"
 #include "wotqs_host.hpp"
 #include "bignum_host.hpp"
@@ -236,8 +237,10 @@ struct bftq_engine {
   HandleList<bftq_thrsa_share> thrsa;            // threshold-RSA fragments
   HandleList<bftq_thdsa_share> thdsa;            // threshold-DSA Y and (k, c) tables; mu also covers the sign calls
   HandleList<bftq_auth_server> auth;             // auth parameters and phase-1 state; mu also covers the respond calls
+  HandleList<bftq_auth_client> auth_client;      // auth client sessions; mu also covers the process calls
   uint32_t* d_p256_base = nullptr;               // K8's fixed-base table of P-256 (public), built on first use
   bftq::k9::AuthGroup* d_auth_group = nullptr;   // K9's group constants (public), built on first use
+  bftq::k9::AuthGroup* d_auth_group_q = nullptr; // K10's constants of q = (p - 1) / 2 (public), built on first use
 };
 
 namespace {
@@ -1669,6 +1672,7 @@ int bftq_pgp_digest_batch(bftq_engine* e, const uint8_t* data_blob, const uint64
 #include "thrsa_host.inc"
 #include "thdsa_host.inc"
 #include "auth_host.inc"
+#include "auth_client_host.inc"
 
 extern "C" {
 // After the .inc files: the handle lists detach handle types defined there.
@@ -1679,6 +1683,7 @@ void bftq_shutdown(bftq_engine* e) {
   e->thrsa.shutdown();
   e->thdsa.shutdown();
   e->auth.shutdown();
+  e->auth_client.shutdown();
   for (auto& kv : e->host_allocs) cudaFreeHost(kv.first);
   for (auto* s : e->slots) {
     if (s->stream) { cudaStreamSynchronize(s->stream); cudaStreamDestroy(s->stream); }
@@ -1691,6 +1696,7 @@ void bftq_shutdown(bftq_engine* e) {
   if (e->d_keys32) cudaFree(e->d_keys32);
   if (e->d_p256_base) cudaFree(e->d_p256_base);
   if (e->d_auth_group) cudaFree(e->d_auth_group);
+  if (e->d_auth_group_q) cudaFree(e->d_auth_group_q);
   cudaDeviceSynchronize();
   for (auto& b : e->scratch.free_list) cudaFree(b.first);
   for (cudaEvent_t ev : e->ed.pending) cudaEventDestroy(ev);

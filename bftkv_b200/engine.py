@@ -383,6 +383,44 @@ class Engine:
                                                             _ptr(rblob), _ptr(roff), n, _ptr(err), _ptr(out), cap, _ptr(out_off)))
         return err[:n], [bytes(out[out_off[i]:out_off[i + 1]]) for i in range(n)]
 
+    def auth_client_create(self, password: bytes, n: int, k: int):
+        """Registers one password-authentication client session (auth.NewClient(cred, n, k)) on the device; returns its handle."""
+        h = C.c_void_p()
+        pb = np.frombuffer(password, np.uint8) if password else np.zeros(1, np.uint8)
+        _lib.check(self._lib.bftq_auth_client_create(self._h, _ptr(pb), len(password), n, k, C.byref(h)))
+        return h
+
+    def auth_client_destroy(self, client):
+        self._lib.bftq_auth_client_destroy(client)
+
+    def auth_client_process_batch(self, clients, client_idx, ops, peer_ids, datas, rands):
+        """Initiate (op -1), ProcessResponse(op, datas[i], peer_ids[i]) (ops 0..2) and GetCipherKey (op -2) on
+        clients[client_idx[i]], one call.  rands[i]: a (256 bytes, Initiate), the a' values of a completing phase-0 item, else
+        b"".  (out_err int32[n], has_map uint8[n], [outputs]); the output buffer is sized from the library's out_need."""
+        n = len(ops)
+        blob, off = self._blob(list(datas))
+        rblob, roff = self._blob(list(rands))
+        tab = (C.c_void_p * max(1, len(clients)))(*[c.value for c in clients])
+        idx = np.ascontiguousarray(client_idx, np.uint32) if n else np.zeros(1, np.uint32)
+        op = np.ascontiguousarray(ops, np.int32) if n else np.zeros(1, np.int32)
+        peers = np.ascontiguousarray(peer_ids, np.uint64) if n else np.zeros(1, np.uint64)
+        out_off = np.zeros(n + 1, np.uint64)
+        err = np.zeros(max(1, n), np.int32)
+        has = np.zeros(max(1, n), np.uint8)
+        need = C.c_uint64(0)
+        cap = 0
+        while True:
+            out = np.zeros(max(1, cap), np.uint8)
+            rc = self._lib.bftq_auth_client_process_batch(self._h, tab, len(clients), _ptr(idx), _ptr(op), _ptr(peers), _ptr(blob), _ptr(off),
+                                                          _ptr(rblob), _ptr(roff), n, _ptr(err), _ptr(has), _ptr(out), cap, _ptr(out_off),
+                                                          C.byref(need))
+            if rc == -3 and need.value > cap:
+                cap = need.value
+                continue
+            _lib.check(rc)
+            break
+        return err[:n], has[:n], [bytes(out[out_off[i]:out_off[i + 1]]) for i in range(n)]
+
     def lagrange_exp_product_batch(self, p: int, q: int, x, ys):
         """auth.calculateSharedSecret: prod_j ys[i][j]^lambda_j mod p.  x: (B,k) ints, ys: B lists of k ints."""
         plen, qlen = (p.bit_length() + 7) // 8, (q.bit_length() + 7) // 8

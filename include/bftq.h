@@ -51,6 +51,9 @@ extern "C" {
 #define BFTQ_ERR_SHARE_NOT_FOUND -14   /* crypto.ErrShareNotFound (threshold DSA: no joint share for this node, or a stale nonce) */
 #define BFTQ_ERR_KEY_NOT_FOUND   -15   /* crypto.ErrKeyNotFound (threshold DSA: phase 3 without a phase 2 for the peer) */
 #define BFTQ_ERR_AUTH_FAILURE    -16   /* bftkv.ErrAuthenticationFailure (password authentication: Ni does not match) */
+#define BFTQ_ERR_NO_AUTH_DATA    -17   /* crypto.ErrNoAuthenticationData (password authentication: no secret for the peer) */
+#define BFTQ_ERR_DECRYPTION_FAILED -18 /* crypto.ErrDecryptionFailed (password authentication: Zi does not open) */
+#define BFTQ_ERR_INSUFFICIENT_SECRETS -19 /* crypto.ErrInsufficientNumberOfSecrets (GetCipherKey before k secrets) */
 
 /* ---- per-item status bytes (SURVEY §8b "Errors") --------------------------------------------
  * The reference collapses every failure to ErrInvalidSignature (crypto_pgp.go:325-327); the shim
@@ -650,6 +653,57 @@ int bftq_auth_server_respond_batch(bftq_engine* e, bftq_auth_server* const* hand
                                    const int32_t* phase, const uint8_t* req_blob, const uint64_t* req_off, const uint8_t* rand_blob,
                                    const uint64_t* rand_off, uint64_t n_items, int32_t* out_err, uint8_t* out_blob, uint64_t out_cap,
                                    uint64_t* out_off);
+
+/* ---- threshold password authentication, client half (crypto/auth/auth.go:239-399, K10) ---------------------------
+ * bftq_auth_client_create is auth.NewClient(cred, n, k), 1 <= k <= n <= 255.  The password goes to the session's device
+ * allocation (header: a, a^-1 mod q, gs; n slots: a'_i, ke and its flag; then the password), zeroed before it
+ * is freed (bftq_auth_client_destroy, bftq_shutdown).  The host keeps public values only: per peer its id, x, Yi, salt,
+ * Xi, Ni and Pi.  The salt's HMAC key block is public and travels with each phase-1 item. */
+typedef struct bftq_auth_client bftq_auth_client;
+int  bftq_auth_client_create(bftq_engine* e, const uint8_t* cred, uint64_t cred_len, uint32_t n, uint32_t k, bftq_auth_client** out);
+void bftq_auth_client_destroy(bftq_auth_client* c);
+
+#define BFTQ_AUTH_INITIATE   (-1)   /* generateX: rand = a, 256 big-endian bytes           -> out = X.Bytes()              */
+                                    /* 0, 1, 2: ProcessResponse(phase, data, peer_id)      -> out = the returned map, if any */
+#define BFTQ_AUTH_CIPHER_KEY (-2)   /* GetCipherKey                                         -> out = 32 bytes               */
+
+/* The calls a Go client makes one at a time, batched: item i applies op[i] to handles[handle_idx[i]] with data
+ * data_blob[data_off[i] .. data_off[i+1]) (the answer of peer_id[i]) and randomness rand_blob[rand_off[i] .. rand_off[i+1]).
+ * The result equals the same calls made one after another in item order; items of different sessions are independent.
+ *   INITIATE     rand = a (256 bytes, as rand.Int(rand.Reader, q)); out = X.Bytes().  A second INITIATE replaces a and keeps
+ *                the secrets, gs and the response counter.
+ *   phase 0      processYi.  An item that leaves at least k secrets completes: gs = prod Yi^lambda_i over every secret, a
+ *                fresh a' per secret from rand (m x 256 bytes, one per secret in first-arrival order, m >= the secrets
+ *                the item leaves; extra bytes are ignored, as is the rand of an item that does not complete), and
+ *                out = the map {peer: Xi}.  A repeated peer replaces its secret (and drops its keys, Ni and Pi).
+ *   phase 1      processBi: Ki = Bi^(a a' mod q), keySched, Ni = MAC(km, Xi, Bi.Bytes()) of the received Bi; every answer
+ *                counts, repeated ones too; the answer that brings the count to the number of secrets returns {peer: Ni}
+ *                (an empty Ni for a peer that never answered) and resets the count.
+ *   phase 2      processZi: Pi = AES-128-GCM(ke).Open(nonce, Zi, Ni); a failure does not count and, as Go's
+ *                `secret.Pi, err = decrypt(...)`, leaves the peer with no Pi (an empty map entry); the count reaching the
+ *                number of secrets returns {peer: Pi}.
+ *   CIPHER_KEY   SHA-256((gs^(a^-1) mod p).Bytes() || pw), 32 bytes.
+ *   other ops    nothing (ProcessResponse's other phases).
+ * A map is u32 count | count x (u64 peer id | u64 length | bytes), big-endian, in the order the secrets first arrived (one
+ * legal order of Go's map); out_has_map[i] = 1 tells Go's non-nil map from nil.  Item i's output is at out_blob[out_off[i] ..
+ * out_off[i+1]).
+ *   out_err[i]   0 | BFTQ_ERR_MALFORMED (parseYi / parseBi / parseZi) | BFTQ_ERR_NO_AUTH_DATA (phase 1 or 2 from a peer with no
+ *                secret) | BFTQ_ERR_DECRYPTION_FAILED | BFTQ_ERR_INSUFFICIENT_SECRETS (CIPHER_KEY before gs).  A failed item
+ *                changes nothing, except that BFTQ_ERR_DECRYPTION_FAILED drops the peer's Pi, as Go does.
+ * BFTQ_ERR_INVALID_ARG before any work, with nothing changed: items of one session with different ops, INITIATE or CIPHER_KEY
+ * twice for one session, a rand of the wrong length, a = 0 mod q (ModInverse fails), more than n distinct phase-0 peers, a
+ * phase 1 or CIPHER_KEY on a session with no a or a phase 1 on a secret with no a' (Go dereferences nil there), or out_cap
+ * below *out_need.  *out_need (the bytes the outputs may take, from public data) is set on every return.
+ * Divergences: phase 2 for a peer whose keys phase 1 never set fails with BFTQ_ERR_DECRYPTION_FAILED (Go opens under an
+ * all-zero key); a nonce that is not 12 bytes fails with BFTQ_ERR_DECRYPTION_FAILED (Go's aead.Open panics); the (n+1)-th
+ * distinct peer is rejected (protocol/client.go multicasts to n nodes only).  Per-call buffers that held a, a', e, f or Ki
+ * are zeroed before the call returns.  A BFTQ_ERR_CUDA / BFTQ_ERR_NOMEM return after the device work began can leave the
+ * device half of the call's sessions partly updated while their host half is not: destroy those sessions. */
+int bftq_auth_client_process_batch(bftq_engine* e, bftq_auth_client* const* handles, uint32_t n_handles, const uint32_t* handle_idx,
+                                   const int32_t* op, const uint64_t* peer_id, const uint8_t* data_blob, const uint64_t* data_off,
+                                   const uint8_t* rand_blob, const uint64_t* rand_off, uint64_t n_items,
+                                   int32_t* out_err, uint8_t* out_has_map, uint8_t* out_blob, uint64_t out_cap, uint64_t* out_off,
+                                   uint64_t* out_need);
 
 /* ---- quorum-descriptor builder (host only; no GPU needed) --------------------------------------
  * The step before the tally: wotqs.ChooseQuorum over the PGP trust graph
