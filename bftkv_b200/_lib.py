@@ -116,6 +116,9 @@ def load():
         "bftq_thdsa_share_destroy": (None, [vp]),
         "bftq_thdsa_share_out_bound": (C.c_uint64, [vp]),
         "bftq_thdsa_sign_batch": (C.c_int, [vp, vp, C.c_uint32, vp, vp, vp, vp, C.c_uint64, vp, vp, vp, C.c_uint64, vp, vp, C.c_uint64, vp]),
+        "bftq_thdsa_proc_create": (C.c_int, [C.c_uint32, vp, C.c_uint64, C.c_uint32, vp, C.c_uint32, C.POINTER(vp)]),
+        "bftq_thdsa_proc_destroy": (None, [vp]),
+        "bftq_thdsa_process_batch": (C.c_int, [vp, vp, C.c_uint32, vp, vp, vp, vp, vp, C.c_uint64, vp, vp, vp, C.c_uint64, vp, vp]),
         "bftq_auth_server_create": (C.c_int, [vp, vp, C.c_uint64, vp, C.c_uint64, C.POINTER(vp)]),
         "bftq_auth_server_destroy": (None, [vp]),
         "bftq_auth_server_out_bound": (C.c_uint64, [vp, C.c_int32]),

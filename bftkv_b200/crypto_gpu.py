@@ -516,6 +516,59 @@ class ThresholdDSA:
         self._shares = {}
 
 
+ErrContinue = "crypto: continue"
+THDSA_REQUEST, THDSA_RESPONSE = -1, 0
+THDSA_PENDING, THDSA_CONTINUE, THDSA_SIGNED, THDSA_FAILED = 0, 1, 2, 3
+
+
+class ThresholdDSAProcess:
+    """The client half of crypto.Threshold for TH_DSA / TH_ECDSA (dsa_core.go dsaProc): MakeRequest and ProcessResponse
+    over a process whose CalculateR and calculateS run on the device.  The process holds public state only.  dgst is
+    hash(tbs) as NewProcess computes it; t and node_ids are the context's.  ErrContinue is returned as a sentinel string."""
+
+    _ERRS = {-8: "threshold dsa: malformed response", -4: ErrNotBuilt}
+
+    def __init__(self, engine: Engine, curve: str, dgst: bytes, t: int, node_ids: Sequence[int]):
+        self.engine = engine
+        self._h = engine.thdsa_proc_create({"dsa": TH_DSA, "p256": TH_ECDSA}[curve], dgst, t, list(node_ids))
+
+    @classmethod
+    def process_batch(cls, engine: Engine, procs: Sequence["ThresholdDSAProcess"], ops: Sequence[int], datas: Sequence[bytes],
+                      peer_ids: Sequence[int]):
+        """Items (procs[i], ops[i], datas[i], peer_ids[i]) in one call, applied as if one at a time in order.  A REQUEST gives
+        ((node ids, request bytes or None), None); a RESPONSE (result or None, None / ErrContinue / an error)."""
+        tab = list({id(p): p for p in procs}.values())
+        pos = {id(p): j for j, p in enumerate(tab)}
+        state, err, outs = engine.thdsa_process_batch([p._h for p in tab], [pos[id(p)] for p in procs], list(ops), list(peer_ids), list(datas))
+        res = []
+        for op, st, e, o in zip(ops, state, err, outs):
+            if st == THDSA_FAILED:
+                res.append((None, cls._ERRS.get(int(e), int(e))))
+            elif op == THDSA_REQUEST:
+                cnt = int.from_bytes(o[:4], "big")
+                ids = [int.from_bytes(o[4 + 8 * j:12 + 8 * j], "big") for j in range(cnt)]
+                req = o[4 + 8 * cnt:]
+                res.append(((ids, req or None), None))
+            elif st == THDSA_SIGNED:
+                res.append((o, None))
+            else:
+                res.append((None, ErrContinue if st == THDSA_CONTINUE else None))
+        return res
+
+    def make_request(self):
+        """MakeRequest(): ((node ids, request or None), err)."""
+        return self.process_batch(self.engine, [self], [THDSA_REQUEST], [b""], [0])[0]
+
+    def process_response(self, data: bytes, peer_id: int):
+        """ProcessResponse(data, peer): (result or None, err)."""
+        return self.process_batch(self.engine, [self], [THDSA_RESPONSE], [data], [peer_id])[0]
+
+    def close(self):
+        if self._h is not None:
+            self.engine.thdsa_proc_destroy(self._h)
+            self._h = None
+
+
 ErrAuthenticationFailure = "authentication failure"
 ErrAuthTooManyAttempts = "crypto: too many attempts"
 AUTH_RETRY_LIMIT = 10

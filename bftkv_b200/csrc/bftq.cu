@@ -23,6 +23,7 @@
 #include "bignum_host.hpp"
 #include "device_secret.hpp"
 #include "wire_host.hpp"
+#include "thdsa_wire.hpp"
 
 #include <algorithm>
 #include <array>
@@ -1444,18 +1445,97 @@ int bftq_modprod_batch(bftq_engine* e, const uint8_t* m_be, uint32_t mlen, uint3
   return a.download();
 }
 
+}  // extern "C"
+namespace {
 // prod_i Y_i^lambda_i mod p with lambda_i = Lagrange(x_i, xs, q): K3 (lambda) -> K5 modexp -> K5 product.
-static int lagrange_exp_product_dev(bftq_engine* e, Arena& a, const uint8_t* p_be, uint32_t plen, const uint8_t* q_be, uint32_t qlen, uint32_t k,
-                                    const int32_t* d_x, const uint8_t* d_y, uint64_t n_items, uint8_t* d_lambda, uint8_t* d_pow, uint8_t* d_dummy_out,
-                                    uint8_t* d_st, uint8_t* d_prod) {
+int lagrange_exp_product_dev(bftq_engine* e, cudaStream_t st, const uint8_t* p_be, uint32_t plen, const uint8_t* q_be, uint32_t qlen, uint32_t k,
+                             const int32_t* d_x, const uint8_t* d_y, uint64_t n_items, uint8_t* d_lambda, uint8_t* d_pow, uint8_t* d_dummy_out,
+                             uint8_t* d_st, uint8_t* d_prod) {
   // lambda only: feed the combine kernel zero shares (d_pow is zero-initialised scratch of sufficient size is not
   // needed: y is read but its product is discarded) — reuse d_y's first bytes as y is only multiplied in.
-  int rc = launch_lagrange_any(e, q_be, qlen, k, d_x, d_lambda /* any readable k*qlen bytes per item */, n_items, d_dummy_out, d_st, d_lambda, a.stream());
+  int rc = launch_lagrange_any(e, q_be, qlen, k, d_x, d_lambda /* any readable k*qlen bytes per item */, n_items, d_dummy_out, d_st, d_lambda, st);
   if (rc) return rc;
-  rc = modexp_any(e, p_be, plen, d_y, d_lambda, qlen, n_items * k, d_pow, a.stream());
+  rc = modexp_any(e, p_be, plen, d_y, d_lambda, qlen, n_items * k, d_pow, st);
   if (rc) return rc;
-  return modprod_any(e, p_be, plen, d_pow, k, n_items, d_prod, a.stream());
+  return modprod_any(e, p_be, plen, d_pow, k, n_items, d_prod, st);
 }
+
+// CalculateR's device scratch for n items of k shares, declared on the call's arena.
+struct DsaRScratch {
+  uint8_t *lam, *pow, *tmp, *prod, *v, *vinv, *rp, *st2;
+  void declare(Arena& a, uint64_t n, uint32_t k, uint32_t plen, uint32_t qlen) {
+    a.out(&lam, (uint8_t*)nullptr, (size_t)n * k * qlen, 0);
+    a.out(&pow, (uint8_t*)nullptr, (size_t)n * k * plen, 0);
+    a.out(&tmp, (uint8_t*)nullptr, (size_t)n * qlen, 0);
+    a.out(&prod, (uint8_t*)nullptr, (size_t)n * plen, 0);
+    a.out(&v, (uint8_t*)nullptr, (size_t)n * qlen, 0);
+    a.out(&vinv, (uint8_t*)nullptr, (size_t)n * qlen, 0);
+    a.out(&rp, (uint8_t*)nullptr, (size_t)n * plen, 0);
+    a.out(&st2, (uint8_t*)nullptr, (size_t)n, 0);
+  }
+};
+// dsaGroupOperations.CalculateR over one group (dsa.go:33-52), device pointers: d_ri n x k x plen (< p), d_vi n x k x qlen,
+// d_out n x qlen, d_st n.  go_inverse: the exponent is Go's v.ModInverse(v, q) (thdsa_go_inverse_kernel: v^-1, or v when
+// there is none); otherwise Fermat's v^(q-2) with status 3 for v = 0 (q prime).  Status 3 also marks a lambda whose
+// denominator has no inverse mod q.
+int dsa_calculate_r_dev(bftq_engine* e, cudaStream_t st, const uint8_t* p_be, uint32_t plen, const uint8_t* q_be, uint32_t qlen, uint32_t k,
+                        const int32_t* d_x, const uint8_t* d_ri, const uint8_t* d_vi, uint64_t n_items, const DsaRScratch& s, bool go_inverse,
+                        uint8_t* d_out, uint8_t* d_st) {
+  CU(cudaMemsetAsync(s.lam, 0, (size_t)n_items * k * qlen, st));
+  // r' = prod R_i^lambda_i mod p                                    (dsa.go:41-46)
+  int rc = lagrange_exp_product_dev(e, st, p_be, plen, q_be, qlen, k, d_x, d_ri, n_items, s.lam, s.pow, s.tmp, d_st, s.prod);
+  if (rc) return rc;
+  // v = sum v_i lambda_i mod q                                      (dsa.go:47-48)
+  rc = launch_lagrange_any(e, q_be, qlen, k, d_x, d_vi, n_items, s.v, s.st2, nullptr, st);
+  if (rc) return rc;
+  // v^-1 mod q                                                      (dsa.go:49)
+  bftq::LagrangeMod<8> M;
+  bftq::make_lagrange_mod<8>(q_be, qlen, M);
+  if (go_inverse) rc = launch(e, "thdsa_go_inverse_kernel", bftq::thdsa_go_inverse_kernel<8>, grid_per_item(n_items, 128), 128, st, M, s.v, n_items, s.vinv);
+  else rc = launch(e, "fermat_inverse_kernel", bftq::fermat_inverse_kernel<8>, grid_per_item(n_items, 128), 128, st, M, s.v, n_items, s.vinv, d_st);
+  if (rc) return rc;
+  // r = r'^(v^-1) mod p                                             (dsa.go:50)
+  rc = modexp_any(e, p_be, plen, s.prod, s.vinv, qlen, n_items, s.rp, st);
+  if (rc) return rc;
+  // r mod q                                                         (dsa.go:51)
+  return launch(e, "mod_small_kernel", bftq::mod_small_kernel<8>, grid_per_item(n_items, 128), 128, st, M, s.rp, plen, n_items, d_out);
+}
+
+struct EcdsaRScratch {
+  uint8_t *lam, *tmp, *v, *vinv, *ok, *st2;
+  uint32_t* jac;
+  void declare(Arena& a, uint64_t n, uint32_t k) {
+    a.out(&lam, (uint8_t*)nullptr, (size_t)n * k * 32, 0);
+    a.out(&tmp, (uint8_t*)nullptr, (size_t)n * 32, 0);
+    a.out(&v, (uint8_t*)nullptr, (size_t)n * 32, 0);
+    a.out(&vinv, (uint8_t*)nullptr, (size_t)n * 32, 0);
+    a.out(&jac, (uint32_t*)nullptr, (size_t)n * k * 24, 0);
+    a.out(&ok, (uint8_t*)nullptr, (size_t)n * k, 0);
+    a.out(&st2, (uint8_t*)nullptr, (size_t)n, 0);
+  }
+};
+// ecdsaGroupOperations.CalculateR on P-256 (ecdsa.go:36-59), device pointers: d_ri n x k x 65, d_vi n x k x 32, d_out n x 32,
+// d_st n: 3 where an R_i is not a curve point or the result is at infinity (r = 0 there).  N is prime, so Fermat's inverse
+// is Go's ModInverse, and v = 0 gives v^-1 = 0, r = 0 as Go's.
+int ecdsa_calculate_r_dev(bftq_engine* e, cudaStream_t st, uint32_t k, const int32_t* d_x, const uint8_t* d_ri, const uint8_t* d_vi, uint64_t n_items,
+                          const EcdsaRScratch& s, uint8_t* d_out, uint8_t* d_st) {
+  CU(cudaMemsetAsync(s.lam, 0, (size_t)n_items * k * 32, st));
+  int rc = launch_lagrange_any(e, kP256N, 32, k, d_x, s.lam, n_items, s.tmp, s.st2, s.lam, st);        // lambda_i mod N
+  if (rc) return rc;
+  rc = launch(e, "p256_scalar_mul_kernel", bftq::p256_scalar_mul_kernel, grid_per_item(n_items * k, 128), 128, st, d_ri, s.lam, n_items * k,
+              s.jac, s.ok);
+  if (rc) return rc;
+  rc = launch_lagrange_any(e, kP256N, 32, k, d_x, d_vi, n_items, s.v, s.st2, nullptr, st);           // v = sum v_i lambda_i
+  if (rc) return rc;
+  bftq::LagrangeMod<8> M;
+  bftq::make_lagrange_mod<8>(kP256N, 32, M);
+  rc = launch(e, "fermat_inverse_kernel", bftq::fermat_inverse_kernel<8>, grid_per_item(n_items, 128), 128, st, M, s.v, n_items, s.vinv, nullptr);
+  if (rc) return rc;
+  return launch(e, "p256_sum_mul_kernel", bftq::p256_sum_mul_kernel, grid_per_item(n_items, 128), 128, st, s.jac, s.ok, k, s.vinv, n_items, d_out,
+                d_st);
+}
+}  // namespace
+extern "C" {
 
 int bftq_lagrange_exp_product_batch(bftq_engine* e, const uint8_t* p_be, uint32_t plen, const uint8_t* q_be, uint32_t qlen, uint32_t k,
                                     const int32_t* x, const uint8_t* y_be, uint64_t n_items, uint8_t* out_be, uint8_t* out_status) {
@@ -1476,7 +1556,7 @@ int bftq_lagrange_exp_product_batch(bftq_engine* e, const uint8_t* p_be, uint32_
   rc = a.upload();
   if (rc) return rc;
   CU(cudaMemsetAsync(d_lam, 0, (size_t)n_items * k * qlen, a.stream()));
-  rc = lagrange_exp_product_dev(e, a, p_be, plen, q_be, qlen, k, d_x, d_y, n_items, d_lam, d_pow, d_tmp, d_st, d_out);
+  rc = lagrange_exp_product_dev(e, a.stream(), p_be, plen, q_be, qlen, k, d_x, d_y, n_items, d_lam, d_pow, d_tmp, d_st, d_out);
   if (rc) return rc;
   return a.download();
 }
@@ -1491,43 +1571,18 @@ int bftq_dsa_calculate_r_batch(bftq_engine* e, const uint8_t* p_be, uint32_t ple
   if (rc) return rc;
   if (n_items == 0) return BFTQ_OK;
   Arena a(e);
-  int32_t* d_x; uint8_t *d_ri, *d_vi, *d_lam, *d_pow, *d_tmp, *d_st, *d_st2, *d_prod, *d_v, *d_vinv, *d_rp, *d_out;
+  int32_t* d_x; uint8_t *d_ri, *d_vi, *d_st, *d_out;
+  DsaRScratch s;
   a.in(&d_x, x, (size_t)n_items * k);
   a.in(&d_ri, ri_be, (size_t)n_items * k * plen);
   a.in(&d_vi, vi_be, (size_t)n_items * k * qlen);
-  a.out(&d_lam, (uint8_t*)nullptr, (size_t)n_items * k * qlen, 0);
-  a.out(&d_pow, (uint8_t*)nullptr, (size_t)n_items * k * plen, 0);
-  a.out(&d_tmp, (uint8_t*)nullptr, (size_t)n_items * qlen, 0);
-  a.out(&d_prod, (uint8_t*)nullptr, (size_t)n_items * plen, 0);
-  a.out(&d_v, (uint8_t*)nullptr, (size_t)n_items * qlen, 0);
-  a.out(&d_vinv, (uint8_t*)nullptr, (size_t)n_items * qlen, 0);
-  a.out(&d_rp, (uint8_t*)nullptr, (size_t)n_items * plen, 0);
-  a.out(&d_st2, (uint8_t*)nullptr, (size_t)n_items, 0);
+  s.declare(a, n_items, k, plen, qlen);
   a.out(&d_st, out_status, (size_t)n_items);
   a.out(&d_out, out_r_be, (size_t)n_items * qlen);
   rc = a.upload();
   if (rc) return rc;
-  cudaStream_t st = a.stream();
-  CU(cudaMemsetAsync(d_lam, 0, (size_t)n_items * k * qlen, st));
-  // r' = prod R_i^lambda_i mod p                                    (dsa.go:41-46)
-  rc = lagrange_exp_product_dev(e, a, p_be, plen, q_be, qlen, k, d_x, d_ri, n_items, d_lam, d_pow, d_tmp, d_st, d_prod);
+  rc = dsa_calculate_r_dev(e, a.stream(), p_be, plen, q_be, qlen, k, d_x, d_ri, d_vi, n_items, s, false, d_out, d_st);
   if (rc) return rc;
-  // v = sum v_i lambda_i mod q                                      (dsa.go:47-48)
-  rc = launch_lagrange_any(e, q_be, qlen, k, d_x, d_vi, n_items, d_v, d_st2, nullptr, st);
-  if (rc) return rc;
-  // v^-1 mod q (q prime: Fermat)                                    (dsa.go:50)
-  {
-    bftq::LagrangeMod<8> M;
-    bftq::make_lagrange_mod<8>(q_be, qlen, M);
-    rc = launch(e, "fermat_inverse_kernel", bftq::fermat_inverse_kernel<8>, grid_per_item(n_items, 128), 128, st, M, d_v, n_items, d_vinv, d_st);
-    if (rc) return rc;
-    // r = r'^(v^-1) mod p                                           (dsa.go:51)
-    rc = modexp_any(e, p_be, plen, d_prod, d_vinv, qlen, n_items, d_rp, st);
-    if (rc) return rc;
-    // r mod q                                                       (dsa.go:52)
-    rc = launch(e, "mod_small_kernel", bftq::mod_small_kernel<8>, grid_per_item(n_items, 128), 128, st, M, d_rp, plen, n_items, d_out);
-    if (rc) return rc;
-  }
   return a.download();
 }
 
@@ -1536,39 +1591,18 @@ int bftq_ecdsa_p256_calculate_r_batch(bftq_engine* e, uint32_t k, const int32_t*
   if (!e || !x || !ri || !vi_be || !out_r_be || !out_status) return fail(BFTQ_ERR_INVALID_ARG, "NULL argument");
   if (k == 0 || k > 255) return fail(BFTQ_ERR_INVALID_ARG, "k must be 1..255");
   if (n_items == 0) return BFTQ_OK;
-  static const uint8_t kN[32] = {0xff, 0xff, 0xff, 0xff, 0x00, 0x00, 0x00, 0x00, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff, 0xff,
-                                 0xbc, 0xe6, 0xfa, 0xad, 0xa7, 0x17, 0x9e, 0x84, 0xf3, 0xb9, 0xca, 0xc2, 0xfc, 0x63, 0x25, 0x51};
   Arena a(e);
-  int32_t* d_x; uint8_t *d_ri, *d_vi, *d_lam, *d_tmp, *d_st, *d_st2, *d_v, *d_vinv, *d_ok, *d_out; uint32_t* d_jac;
+  int32_t* d_x; uint8_t *d_ri, *d_vi, *d_st, *d_out;
+  EcdsaRScratch s;
   a.in(&d_x, x, (size_t)n_items * k);
   a.in(&d_ri, ri, (size_t)n_items * k * 65);
   a.in(&d_vi, vi_be, (size_t)n_items * k * 32);
-  a.out(&d_lam, (uint8_t*)nullptr, (size_t)n_items * k * 32, 0);
-  a.out(&d_tmp, (uint8_t*)nullptr, (size_t)n_items * 32, 0);
-  a.out(&d_v, (uint8_t*)nullptr, (size_t)n_items * 32, 0);
-  a.out(&d_vinv, (uint8_t*)nullptr, (size_t)n_items * 32, 0);
-  a.out(&d_jac, (uint32_t*)nullptr, (size_t)n_items * k * 24, 0);
-  a.out(&d_ok, (uint8_t*)nullptr, (size_t)n_items * k, 0);
-  a.out(&d_st2, (uint8_t*)nullptr, (size_t)n_items, 0);
+  s.declare(a, n_items, k);
   a.out(&d_st, out_status, (size_t)n_items);
   a.out(&d_out, out_r_be, (size_t)n_items * 32);
   int rc = a.upload();
   if (rc) return rc;
-  cudaStream_t st = a.stream();
-  CU(cudaMemsetAsync(d_lam, 0, (size_t)n_items * k * 32, st));
-  rc = launch_lagrange_any(e, kN, 32, k, d_x, d_lam, n_items, d_tmp, d_st2, d_lam, st);          // lambda_i mod N
-  if (rc) return rc;
-  rc = launch(e, "p256_scalar_mul_kernel", bftq::p256_scalar_mul_kernel, grid_per_item(n_items * k, 128), 128, st, d_ri, d_lam, n_items * k,
-              d_jac, d_ok);
-  if (rc) return rc;
-  rc = launch_lagrange_any(e, kN, 32, k, d_x, d_vi, n_items, d_v, d_st2, nullptr, st);             // v = sum v_i lambda_i
-  if (rc) return rc;
-  bftq::LagrangeMod<8> M;
-  bftq::make_lagrange_mod<8>(kN, 32, M);
-  rc = launch(e, "fermat_inverse_kernel", bftq::fermat_inverse_kernel<8>, grid_per_item(n_items, 128), 128, st, M, d_v, n_items, d_vinv, nullptr);
-  if (rc) return rc;
-  rc = launch(e, "p256_sum_mul_kernel", bftq::p256_sum_mul_kernel, grid_per_item(n_items, 128), 128, st, d_jac, d_ok, k, d_vinv, n_items, d_out,
-              d_st);
+  rc = ecdsa_calculate_r_dev(e, a.stream(), k, d_x, d_ri, d_vi, n_items, s, d_out, d_st);
   if (rc) return rc;
   return a.download();
 }
@@ -1673,6 +1707,7 @@ int bftq_pgp_digest_batch(bftq_engine* e, const uint8_t* data_blob, const uint64
 #include "thdsa_host.inc"
 #include "auth_host.inc"
 #include "auth_client_host.inc"
+#include "thdsa_proc_host.inc"
 
 extern "C" {
 // After the .inc files: the handle lists detach handle types defined there.

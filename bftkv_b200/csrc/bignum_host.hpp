@@ -4,6 +4,7 @@
 #include <cstddef>
 #include <cstdint>
 #include <cstring>
+#include <vector>
 
 namespace bftq {
 namespace hostbig {
@@ -48,6 +49,27 @@ inline void from_be(UBig& a, const uint8_t* be, size_t len) {   // len bytes big
 }
 inline void to_words(const UBig& a, uint32_t* w, int nw) {
   for (int i = 0; i < nw; i++) w[i] = (uint32_t)(a.w[i / 2] >> (32 * (i & 1)));
+}
+
+// b mod m as mlen big-endian bytes: b public, any length; m_be without leading zeros, mlen <= 256.
+inline std::vector<uint8_t> be_mod(const uint8_t* b, uint64_t l, const uint8_t* m_be, uint32_t mlen) {
+  while (l && !*b) { b++; l--; }
+  std::vector<uint8_t> out(mlen, 0);
+  if (l < mlen || (l == mlen && memcmp(b, m_be, mlen) < 0)) {
+    if (l) memcpy(out.data() + mlen - l, b, l);
+    return out;
+  }
+  UBig P, acc;
+  from_be(P, m_be, mlen);
+  memset(&acc, 0, sizeof(acc));
+  for (uint64_t i = 0; i < l; i++) {             // Horner over bytes: acc = 256 acc + b[i] mod m
+    acc = shl_mod(acc, P, 8);
+    acc.w[0] += b[i];
+    for (int j = 0; acc.w[j] < b[i] && j + 1 < kHL; j++) { if (++acc.w[j + 1]) break; }
+    while (ge(acc, P)) sub(acc, P);              // b[i] < 256: more than one subtraction only when m < 256
+  }
+  for (uint32_t i = 0; i < mlen; i++) out[mlen - 1 - i] = (uint8_t)(acc.w[i / 8] >> (8 * (i % 8)));
+  return out;
 }
 
 // -n^-1 mod 2^32 / 2^64 for odd n (Montgomery's n0inv), by Newton iteration: each step doubles the correct low bits

@@ -355,6 +355,42 @@ class Engine:
                                                    _ptr(nblob), _ptr(noff), _ptr(has), n, _ptr(err), _ptr(out), cap, _ptr(out_off)))
         return err[:n], [bytes(out[out_off[i]:out_off[i + 1]]) for i in range(n)]
 
+    def thdsa_proc_create(self, algo: int, dgst: bytes, t: int, node_ids):
+        """A threshold-DSA client process (dsaContext.NewProcess; algo 2 = TH_DSA, 3 = TH_ECDSA), host memory only."""
+        h = C.c_void_p()
+        db = np.frombuffer(dgst, np.uint8) if dgst else np.zeros(1, np.uint8)
+        ids = np.ascontiguousarray(list(node_ids) or [0], np.uint64)
+        _lib.check(self._lib.bftq_thdsa_proc_create(algo, _ptr(db), len(dgst), t, _ptr(ids), len(node_ids), C.byref(h)))
+        return h
+
+    def thdsa_proc_destroy(self, proc):
+        self._lib.bftq_thdsa_proc_destroy(proc)
+
+    def thdsa_process_batch(self, procs, proc_idx, ops, peer_ids, datas):
+        """MakeRequest (op -1) and ProcessResponse(datas[i], peer_ids[i]) (op 0) on procs[proc_idx[i]], one call.
+        (out_state int32[n], out_err int32[n], [outputs]); the output buffer is sized from the library's out_need."""
+        n = len(ops)
+        blob, off = self._blob(list(datas))
+        tab = (C.c_void_p * max(1, len(procs)))(*[p.value for p in procs])
+        idx = np.ascontiguousarray(proc_idx, np.uint32) if n else np.zeros(1, np.uint32)
+        op = np.ascontiguousarray(ops, np.int32) if n else np.zeros(1, np.int32)
+        peers = np.ascontiguousarray(peer_ids, np.uint64) if n else np.zeros(1, np.uint64)
+        out_off = np.zeros(n + 1, np.uint64)
+        state = np.zeros(max(1, n), np.int32)
+        err = np.zeros(max(1, n), np.int32)
+        need = C.c_uint64(0)
+        cap = 0
+        while True:
+            out = np.zeros(max(1, cap), np.uint8)
+            rc = self._lib.bftq_thdsa_process_batch(self._h, tab, len(procs), _ptr(idx), _ptr(op), _ptr(peers), _ptr(blob), _ptr(off), n,
+                                                    _ptr(state), _ptr(err), _ptr(out), cap, _ptr(out_off), C.byref(need))
+            if rc == -3 and need.value > cap:
+                cap = need.value
+                continue
+            _lib.check(rc)
+            break
+        return state[:n], err[:n], [bytes(out[out_off[i]:out_off[i + 1]]) for i in range(n)]
+
     def auth_server_create(self, params: bytes, proof: bytes):
         """Registers one password-authentication server (auth.NewServer(params, proof)) on the device; returns its handle."""
         h = C.c_void_p()

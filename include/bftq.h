@@ -402,6 +402,48 @@ int bftq_thdsa_sign_batch(bftq_keyring* kr, bftq_thdsa_share* const* shares, uin
                           const uint8_t* req_blob, const uint64_t* req_off, const uint64_t* peer_id, uint64_t self_id,
                           const uint8_t* nonce_blob, const uint64_t* nonce_off, const uint8_t* has_nonce, uint64_t n_items,
                           int32_t* out_err, uint8_t* out_blob, uint64_t out_cap, uint64_t* out_off);
+/* ---- K8, client half: dsaProc (crypto/threshold/dsa/dsa_core.go:269-403) -----------------------------------------------
+ * bftq_thdsa_proc_create is dsaContext.NewProcess: algo = BFTQ_THDSA_DSA / _ECDSA, dgst = hash(tbs) as Go computes it, t and
+ * node_ids the context's (ctx.t, ctx.nodes: what the first MakeRequest returns).  2t > 255 is BFTQ_ERR_UNSUPPORTED_KEY.  A
+ * process holds public state only (the digest, t, the node list, the kmap, the partial signatures, m, r, the phase and the
+ * result), in host memory: no key material, no device allocation, no engine.  One process must not be used by two calls at
+ * once, as Go's dsaProc. */
+typedef struct bftq_thdsa_proc bftq_thdsa_proc;
+int  bftq_thdsa_proc_create(uint32_t algo, const uint8_t* dgst, uint64_t dgst_len, uint32_t t, const uint64_t* node_ids, uint32_t n_nodes,
+                            bftq_thdsa_proc** out);
+void bftq_thdsa_proc_destroy(bftq_thdsa_proc* p);
+
+#define BFTQ_THDSA_REQUEST   (-1)   /* MakeRequest                      */
+#define BFTQ_THDSA_RESPONSE  0      /* ProcessResponse(data, peer_id)   */
+#define BFTQ_THDSA_PENDING   0      /* out_state: (nil, nil)            */
+#define BFTQ_THDSA_CONTINUE  1      /*            crypto.ErrContinue    */
+#define BFTQ_THDSA_SIGNED    2      /*            the r || s result     */
+#define BFTQ_THDSA_FAILED    3      /*            out_err[i]            */
+/* The calls a Go client makes one at a time, batched: item i applies op[i] to procs[proc_idx[i]], a RESPONSE with the answer
+ * data_blob[data_off[i] .. data_off[i+1]) of peer_id[i].  The result equals the same calls made one after another in item
+ * order; items of different processes are independent.  Item i's output is at out_blob[out_off[i] .. out_off[i+1]).
+ *   REQUEST   u32 count | count x u64 node id (the node list, which then resets), then the request: phase 1
+ *             serializeSignRequest(nil, nil, kmap) with the ids in first-insertion order (one legal order of Go's map), phase 2
+ *             01 || chunk(m) || chunk(r), else nothing (Go's nil).
+ *   RESPONSE  out_state; SIGNED writes formatDSA(r, s, q).  The peer joins the node list before any parsing.
+ *             phase 0  parseJointShare; the phase advances when the count of the last-listed id reaches 2t.
+ *             phase 1  the 2t-th partial signature runs CalculateR and OS2I with its own group (DSA OS2I: dgst[:|q| bytes]).
+ *             phase 2  the 2t-th runs calculateS mod its own q, then formatDSA; every later RESPONSE returns the same result.
+ *             x is Go's int(u64); equal abscissae are skipped in the Lagrange coefficients.  v.ModInverse(v, q) is Go's:
+ *             v^-1 when gcd(v, q) = 1, else v itself (DSA r = 1 for v = 0); ECDSA r = 0 for v = 0 or a sum at infinity.
+ *   out_err[i]  0 | BFTQ_ERR_MALFORMED (framing: the item changes the node list only; or where Go panics: an R_i that
+ *               elliptic.Unmarshal rejects, a Lagrange denominator with no inverse mod q, a digest shorter than the order, an r
+ *               longer than the phase-2 q) | BFTQ_ERR_UNSUPPORTED_KEY (an x outside int32, or a completing answer whose group
+ *               is neither DSA with p odd of exactly 1024 / 2048 bits and q odd, 1 < q < 2^256, nor exactly P-256: the item
+ *               changes nothing, and the shim replays the process on Go).  A completion that fails leaves the process failed:
+ *               it and every later item of the process return the same code.
+ * *out_need (bytes the outputs may take, from public sizes) is set on every return; out_cap below it is BFTQ_ERR_INVALID_ARG
+ * before any work, with nothing changed, as are a bad index or op.  A BFTQ_ERR_CUDA / BFTQ_ERR_NOMEM return can leave the
+ * call's processes advanced past what any output shows: destroy them. */
+int bftq_thdsa_process_batch(bftq_engine* e, bftq_thdsa_proc* const* procs, uint32_t n_procs, const uint32_t* proc_idx,
+                             const int32_t* op, const uint64_t* peer_id, const uint8_t* data_blob, const uint64_t* data_off,
+                             uint64_t n_items, int32_t* out_state, int32_t* out_err, uint8_t* out_blob, uint64_t out_cap,
+                             uint64_t* out_off, uint64_t* out_need);
 /* AuthClient.calculateSharedSecret (crypto/auth/auth.go:386-399) and the first half of CalculateR:
  * out[i] = prod_j y[i][j]^lambda_j mod p,  lambda_j = sss.Lagrange(x[i][j], x[i][*], q).
  * p: plen = 128/256 bytes; q: any odd modulus up to 256 bytes (auth uses q = (p-1)/2). */
