@@ -126,6 +126,8 @@ def load():
         "bftq_auth_client_create": (C.c_int, [vp, vp, C.c_uint64, C.c_uint32, C.c_uint32, C.POINTER(vp)]),
         "bftq_auth_client_destroy": (None, [vp]),
         "bftq_auth_client_process_batch": (C.c_int, [vp, vp, C.c_uint32, vp, vp, vp, vp, vp, vp, vp, C.c_uint64, vp, vp, vp, C.c_uint64, vp, vp]),
+        "bftq_data_encrypt_batch": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_uint64, C.c_uint64, vp, C.c_uint64, vp, vp, vp]),
+        "bftq_data_decrypt_batch": (C.c_int, [vp, vp, vp, vp, vp, C.c_uint64, vp, C.c_uint64, vp, vp, vp]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(lib, name)       # AttributeError here = header/library mismatch: fail loudly

@@ -726,3 +726,37 @@ class AuthClient:
         if self._h is not None:
             self.engine.auth_client_destroy(self._h)
             self._h = None
+
+
+ErrUnexpectedEOF = "unexpected EOF"                        # io.ErrUnexpectedEOF: the literal body ends early
+ErrMalformedMessage = "openpgp: malformed message (the reference's Decrypt panics on it, or fails reading a cut-short body)"
+_DATA_ERRORS = {-8: ErrMalformedMessage, -10: ErrUnexpectedEOF, -11: ErrMessageUnsupported, -12: ErrMDC, -18: ErrDecryptionFailed}
+
+
+class DataEncryption:
+    """crypto.DataEncryption (crypto/crypto.go:73-76, crypto_pgp.go:525-554) on the device: Encrypt is x/crypto's
+    SymmetricallyEncrypt byte for byte, Decrypt its ReadMessage.  `rand(n)` supplies Go's random bytes (default
+    os.urandom, injectable for tests): 40 per Encrypt, salt, session key and IV.  Results are (value, err) pairs with the
+    reference's errors; where Go would never return (a wrong key) the error is ErrDecryptionFailed, and where it would
+    panic (a malformed message) ErrMalformedMessage, which also stands for a SEIPD body cut short (Go: ReadAll's read
+    error)."""
+
+    def __init__(self, engine: Engine, rand=None):
+        import os
+        self.engine = engine
+        self._rand = rand if rand is not None else os.urandom
+
+    def encrypt_batch(self, keys: Sequence[bytes], plains: Sequence[bytes]):
+        rands = [self._rand(40) for _ in plains]
+        err, outs = self.engine.data_encrypt_batch(list(keys), list(plains), rands)
+        return [(o, None) if e == 0 else (None, _DATA_ERRORS.get(int(e), int(e))) for e, o in zip(err, outs)]
+
+    def decrypt_batch(self, keys: Sequence[bytes], ciphers: Sequence[bytes]):
+        err, outs = self.engine.data_decrypt_batch(list(keys), list(ciphers))
+        return [(o, None) if e == 0 else (None, _DATA_ERRORS.get(int(e), int(e))) for e, o in zip(err, outs)]
+
+    def encrypt(self, key: bytes, plain: bytes):
+        return self.encrypt_batch([key], [plain])[0]
+
+    def decrypt(self, key: bytes, cipher: bytes):
+        return self.decrypt_batch([key], [cipher])[0]

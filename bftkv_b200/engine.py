@@ -457,6 +457,61 @@ class Engine:
             break
         return err[:n], has[:n], [bytes(out[out_off[i]:out_off[i + 1]]) for i in range(n)]
 
+    @staticmethod
+    def _secret_blob(items):
+        """A writable copy of the items as one blob (zeroed by the caller after the call) and its offsets."""
+        off = np.zeros(len(items) + 1, np.uint64)
+        off[1:] = np.cumsum([len(b) for b in items], dtype=np.uint64) if items else []
+        blob = np.zeros(max(1, int(off[-1])), np.uint8)
+        for i, b in enumerate(items):
+            blob[int(off[i]):int(off[i + 1])] = np.frombuffer(bytes(b), np.uint8)
+        return blob, off
+
+    def _data_call(self, fn, n, cap, *args):
+        """One K11 call with an output buffer of cap bytes, retried once with *out_need if that is short."""
+        out_off = np.zeros(n + 1, np.uint64)
+        err = np.zeros(max(1, n), np.int32)
+        need = C.c_uint64(0)
+        while True:
+            out = np.zeros(max(1, cap), np.uint8)
+            rc = fn(self._h, *args, _ptr(out), cap, _ptr(out_off), C.byref(need), _ptr(err))
+            if rc == -3 and need.value > cap:
+                cap = need.value
+                continue
+            _lib.check(rc)
+            return err[:n], [bytes(out[out_off[i]:out_off[i + 1]]) for i in range(n)]
+
+    def data_encrypt_batch(self, keys, plains, rands):
+        """DataEncryption.Encrypt(keys[i], plains[i]) with Go's 40 random bytes rands[i] (salt, session key, IV):
+        (out_err int32[n], [messages]).  The host copies of the keys and the randomness are zeroed before returning."""
+        n = len(plains)
+        assert len(keys) == n and len(rands) == n and all(len(r) == 40 for r in rands)
+        kblob, koff = self._secret_blob(list(keys))
+        pblob, poff = self._secret_blob(list(plains))
+        rblob, _ = self._secret_blob(list(rands))
+        # a bound on the message length (value + 3 framing bytes per partial chunk of at most 2^14 bytes + 139 bytes of
+        # packets and fixed chunks), so the first call fits; the library's *out_need still decides
+        cap = sum(len(p) + 3 * (len(p) // 16384) + 139 for p in plains)
+        try:
+            return self._data_call(self._lib.bftq_data_encrypt_batch, n, cap, _ptr(kblob), _ptr(koff), _ptr(pblob), _ptr(poff), _ptr(rblob), 40 * n, n)
+        finally:
+            kblob[:] = 0
+            pblob[:] = 0
+            rblob[:] = 0
+
+    def data_decrypt_batch(self, keys, ciphers):
+        """DataEncryption.Decrypt(keys[i], ciphers[i]): (out_err int32[n], [plain texts]).  The host copy of the keys is
+        zeroed before returning."""
+        n = len(ciphers)
+        assert len(keys) == n
+        kblob, koff = self._secret_blob(list(keys))
+        cblob, coff = self._blob(list(ciphers))
+        try:
+            # the plain texts are shorter than the messages, so the first call fits
+            return self._data_call(self._lib.bftq_data_decrypt_batch, n, int(coff[-1]), _ptr(kblob), _ptr(koff), _ptr(cblob), _ptr(coff), n)
+        finally:
+            kblob[:] = 0
+
     def lagrange_exp_product_batch(self, p: int, q: int, x, ys):
         """auth.calculateSharedSecret: prod_j ys[i][j]^lambda_j mod p.  x: (B,k) ints, ys: B lists of k ints."""
         plen, qlen = (p.bit_length() + 7) // 8, (q.bit_length() + 7) // 8

@@ -747,6 +747,39 @@ int bftq_auth_client_process_batch(bftq_engine* e, bftq_auth_client* const* hand
                                    int32_t* out_err, uint8_t* out_has_map, uint8_t* out_blob, uint64_t out_cap, uint64_t* out_off,
                                    uint64_t* out_need);
 
+/* ---- DataEncryption (K11: crypto_pgp.go:532-554) ---------------------------------------------------------------------
+ * Passphrase encryption of stored values, batched.  Item i's key is key_blob[key_off[i] .. key_off[i+1]) (any length).
+ *
+ * bftq_data_encrypt_batch: Encrypt(key, plain) as x/crypto's SymmetricallyEncrypt(w, key, nil, nil) + Write(plain) + Close
+ * write it, byte for byte: an SKESK (v4, AES-128, iterated-and-salted S2K over SHA-256 with count byte 0x60, the session
+ * key wrapped under the S2K key) and a SEIPD packet holding a text literal packet (empty name, time 0) and the MDC, with
+ * Go's partial-length chunks.  rand: rand_len = 40 x n bytes, item i's at rand[40 i ..]: salt (8), session key (16),
+ * IV (16), in the order Go reads its random source.  Item i's message goes to out_blob[out_off[i] .. out_off[i+1]); its
+ * length is a function of the plain text's length only.  out_err[i] is 0.
+ *
+ * bftq_data_decrypt_batch: Decrypt(key, cipher) as ReadMessage's symmetric half + ReadAll.  The plain text goes to
+ * out_blob[out_off[i] .. out_off[i+1]) (empty unless out_err[i] is 0).
+ *   out_err[i]  0 | BFTQ_ERR_DECRYPTION_FAILED (no SKESK gives a key that passes the quick check: Go's prompt is asked
+ *               forever) | BFTQ_ERR_MDC (the MDC packet is missing or does not match) | BFTQ_ERR_MESSAGE_BODY (the literal
+ *               body ends early) | BFTQ_ERR_MALFORMED (framing, no SKESK, no SEIPD, a stream too short for the prefix or
+ *               the MDC: Go panics on the nil message; divergence: a SEIPD body cut short, where Go returns ReadAll's
+ *               read error) | BFTQ_ERR_UNSUPPORTED (compressed or signed inner data, tag 9, a
+ *               PKESK, S2K modes other than 0 / 1 / 3 or hashes other than SHA-256, a SKESK that is not v4 AES, a 3DES or
+ *               CAST5 key-encryption cipher, more than 16 SKESKs, packets after the SEIPD: the shim runs Go).
+ *   A SKESK whose unwrapped cipher byte is unknown or has the wrong key length is skipped, as in Go.  Divergence: an
+ *   unwrapped 3DES or CAST5 key is skipped too, where Go would try it.
+ *
+ * Both: every BFTQ_ERR_INVALID_ARG (NULL arguments, bad offsets, a rand of the wrong length, a key of 2^32 bytes or more,
+ * out_cap below *out_need) is returned before any device work, with no output written.  *out_need (the exact output
+ * length for encrypt, a bound for decrypt, from lengths only) is set on every return.  The keys, the S2K outputs, the
+ * session keys and the plain texts are on the device only in a per-call buffer zeroed before the call returns. */
+int bftq_data_encrypt_batch(bftq_engine* e, const uint8_t* key_blob, const uint64_t* key_off, const uint8_t* plain_blob,
+                            const uint64_t* plain_off, const uint8_t* rand, uint64_t rand_len, uint64_t n_items, uint8_t* out_blob,
+                            uint64_t out_cap, uint64_t* out_off, uint64_t* out_need, int32_t* out_err);
+int bftq_data_decrypt_batch(bftq_engine* e, const uint8_t* key_blob, const uint64_t* key_off, const uint8_t* cipher_blob,
+                            const uint64_t* cipher_off, uint64_t n_items, uint8_t* out_blob, uint64_t out_cap, uint64_t* out_off,
+                            uint64_t* out_need, int32_t* out_err);
+
 /* ---- quorum-descriptor builder (host only; no GPU needed) --------------------------------------
  * The step before the tally: wotqs.ChooseQuorum over the PGP trust graph
  * (quorum/wotqs/wotqs.go:36-127, node/graph/graph.go:46-75,117-125,279-393,420-438).  The shim
