@@ -84,6 +84,7 @@ def load():
         "bftq_keyring_certifiers": (C.c_int, [vp, C.c_uint64, vp, C.c_uint32, u32p]),
         "bftq_signature_verify_batch": (C.c_int, [vp, vp, vp, vp, vp, C.c_uint64, vp]),
         "bftq_signature_verify_with_cert_batch": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, C.c_uint64, vp]),
+        "bftq_signature_sign_batch": (C.c_int, [vp, vp, vp, vp, C.c_uint64, vp, vp]),
         "bftq_message_verify_batch": (C.c_int, [vp, vp, vp, C.c_uint64, vp, vp, vp, vp, vp, vp, vp]),
         "bftq_message_decrypt_batch": (C.c_int, [vp, vp, vp, C.c_uint64, vp, vp, vp, vp, vp, vp, vp]),
         "bftq_keyring_add_private": (C.c_int, [vp, vp, C.c_uint64, u32p]),

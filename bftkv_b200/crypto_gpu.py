@@ -2,7 +2,7 @@
 
 Names and argument meaning follow the reference (so tests read like the reference's own):
   crypto.Keyring              crypto/crypto.go:35-41      -> Keyring.register / remove / get_keyring
-  crypto.Signature            crypto/crypto.go:50-58      -> Signature.verify / verify_with_certificate / signers
+  crypto.Signature            crypto/crypto.go:50-58      -> Signature.sign / verify / verify_with_certificate / signers
   crypto.CollectiveSignature  crypto/crypto.go:66-71      -> CollectiveSignature.verify / combine / signers
   quorum.Quorum               quorum/quorum.go:18-25      -> Quorum.is_quorum / is_threshold / is_sufficient / reject
 Errors are the reference's sentinels (crypto/crypto.go:13-33): every verification failure is
@@ -26,6 +26,9 @@ ErrMessageBody = "message body / nonce error"
 ErrMessageUnsupported = "unsupported message form (compressed data)"
 ErrNotBuilt = "gpu: key size / curve not built into libbftq (the shim re-runs the item on crypto/pgp)"
 ErrMDC = "openpgp: invalid signature: hash mismatch"        # seMDCReader.Close's SignatureError, returned by ReadAll as is
+ErrCertificateNotFound = "crypto: certifiate not found"            # the reference's spelling (crypto/crypto.go)
+ErrSigningFailed = "crypto: failed to sign"
+SIGN_PACKET_BYTES = 287                                     # BFTQ_SIGN_PACKET_BYTES
 _ERR = {0: None, -6: ErrInvalidSignature, -7: ErrInsufficientNumberOfSignatures, -8: ErrDecryptionFailed, -9: ErrInvalidTransportSecurityData,
         -10: ErrMessageBody, -11: ErrMessageUnsupported, -12: ErrMDC}
 _ERR_SIG = dict(_ERR)
@@ -138,10 +141,39 @@ class Keyring:
 
 
 class Signature:
-    """crypto.Signature's verification half (crypto_pgp.go:319-344,373-390)."""
+    """crypto.Signature (crypto_pgp.go:319-390): signing with the keyring's private key, and verification."""
 
     def __init__(self, keyring: Keyring):
         self.keyring, self._lib = keyring, _lib.load()
+
+    def sign_batch(self, tbs: Sequence[bytes], ctimes: Sequence[int]):
+        """PGPSignature.Sign over many tbs (bftq_signature_sign_batch): secring[0]'s primary key signs item i with creation
+        time ctimes[i].  -> (errs, packets): errs[i] None or ErrSigningFailed, packets[i] the signature packet
+        (SignaturePacket.Data) or None.  A call-level error (ErrCertificateNotFound's code -20, BFTQ_ERR_UNSUPPORTED: the
+        shim signs on crypto/pgp) raises BftqError."""
+        n = len(tbs)
+        if len(ctimes) != n:
+            raise ValueError("sign_batch: one creation time per tbs")
+        tb, to = _blob(tbs)
+        ct = np.asarray(list(ctimes) or [0], np.uint32)
+        out = np.zeros(max(n, 1) * SIGN_PACKET_BYTES, np.uint8)
+        err = np.zeros(max(n, 1), np.int32)
+        p = lambda a: C.c_void_p(a.ctypes.data)
+        _lib.check(self._lib.bftq_signature_sign_batch(self.keyring._h, p(tb), p(to), p(ct), n, p(out), p(err)))
+        errs = [None if e == 0 else ErrSigningFailed for e in err[:n]]
+        packets = [bytes(out[i * SIGN_PACKET_BYTES:(i + 1) * SIGN_PACKET_BYTES]) if e is None else None for i, e in enumerate(errs)]
+        return errs, packets
+
+    def sign(self, tbs: bytes, ctime: Optional[int] = None):
+        """Go's Sign: -> (packet, err), with time.Now()'s seconds as the default creation time."""
+        import time
+        try:
+            errs, packets = self.sign_batch([tbs], [int(time.time()) if ctime is None else ctime])
+        except _lib.BftqError as ex:
+            if ex.code == -20:
+                return None, ErrCertificateNotFound
+            raise
+        return packets[0], errs[0]
 
     def verify_batch(self, tbs: Sequence[bytes], sig_data: Sequence[bytes], certs: Optional[Sequence[bytes]] = None):
         n = len(tbs)

@@ -19,6 +19,7 @@
 #include "auth_server.cuh"
 #include "auth_client.cuh"
 #include "data_encrypt.cuh"
+#include "rsa_sign.cuh"
 #include "pgp_host.hpp"
 #include "wotqs_host.hpp"
 #include "bignum_host.hpp"
@@ -1710,6 +1711,7 @@ int bftq_pgp_digest_batch(bftq_engine* e, const uint8_t* data_blob, const uint64
 #include "auth_client_host.inc"
 #include "thdsa_proc_host.inc"
 #include "data_host.inc"
+#include "sign_host.inc"
 
 extern "C" {
 // After the .inc files: the handle lists detach handle types defined there.

@@ -94,6 +94,36 @@ __device__ __forceinline__ void crt_half(uint32_t (&res)[8], const uint32_t (&c_
   r32::cond_sub<W, true>(res, m, r, gbase);
 }
 
+// mm = c^d mod n (< n) by CRT with the private key `key`: c given as its two 1024-bit halves, mm in the W = 16 layout.
+// The one copy of the private-key operation: K6a decrypts with it, K12 (rsa_sign.cuh) signs.
+template <int BLOCK>
+__device__ __forceinline__ void rsa_crt(uint32_t (&mm)[16], const uint32_t (&c_lo)[8], const uint32_t (&c_hi)[8], const RsaPriv32* __restrict__ key,
+                                        uint32_t (*tab)[8][BLOCK], const int r, const int gbase) {
+  uint32_t m1[8], m2[8];
+  crt_half<BLOCK>(m1, c_lo, c_hi, key->p, key->r2p, key->dp, __ldg(&key->p0inv), tab, r, gbase);
+  crt_half<BLOCK>(m2, c_lo, c_hi, key->q, key->r2q, key->dq, __ldg(&key->q0inv), tab, r, gbase);
+  // Garner with RFC 4880's u = p^-1 mod q:  h = (m2 - m1) u mod q,  m = m1 + p h  (< n)
+  uint32_t q[8], uq[8], a[8], d[8], h[8];
+  const uint32_t q0inv = __ldg(&key->q0inv);
+#pragma unroll
+  for (int j = 0; j < 8; j++) { q[j] = __ldg(key->q + r * 8 + j); uq[j] = __ldg(key->uq + r * 8 + j); a[j] = m1[j]; }
+  r32::cond_sub<8, true>(a, q, r, gbase);                 // m1 < p < 2q
+  const uint32_t bt = r32::group_sub(d, m2, a, r, gbase);
+  uint32_t dq_[8];
+  r32::group_add(dq_, d, q, r, gbase);
+  r32::select_mask(d, dq_, bt);
+  mmul(h, d, uq, q, q0inv, r, gbase);
+  r32::cond_sub<8, true>(h, q, r, gbase);
+  uint32_t h16[16], m16[16], nn[16], pn[16], ph[16];
+  widen(h, h16, r, gbase);
+  widen(m1, m16, r, gbase);
+#pragma unroll
+  for (int j = 0; j < 16; j++) { nn[j] = __ldg(key->n + r * 16 + j); pn[j] = __ldg(key->pn + r * 16 + j); }
+  mmul(ph, pn, h16, nn, __ldg(&key->n0inv), r, gbase);   // p h mod n, almost reduced
+  r32::cond_sub<16, true>(ph, nn, r, gbase);
+  r32::group_add(mm, ph, m16, r, gbase);
+}
+
 // One 4-lane group per item.  c_be: n_items x 256 bytes (the PKESK MPI, left-padded; c <= n checked by the host),
 // slot: key slot per item.  out_info: kDec* | cipher << 8 | key length << 16; out_key: n_items x 32 bytes, the first
 // min(key length, 32) bytes of the session key, zero beyond.
@@ -113,31 +143,10 @@ rsa_crt_decrypt_kernel(const RsaPriv32* __restrict__ keys, const uint32_t* __res
     const uint64_t item = valid ? item_raw : n_items - 1;
     const RsaPriv32* __restrict__ key = keys + __ldg(slot + item);
     const uint8_t* cp = c_be + item * 256u;
-    uint32_t c_lo[8], c_hi[8], m1[8], m2[8];
+    uint32_t c_lo[8], c_hi[8], mm[16];
 #pragma unroll
     for (int j = 0; j < 8; j++) { c_lo[j] = be_word(cp, r * 8 + j); c_hi[j] = be_word(cp, 32 + r * 8 + j); }
-    crt_half<BLOCK>(m1, c_lo, c_hi, key->p, key->r2p, key->dp, __ldg(&key->p0inv), tab, r, gbase);
-    crt_half<BLOCK>(m2, c_lo, c_hi, key->q, key->r2q, key->dq, __ldg(&key->q0inv), tab, r, gbase);
-    // Garner with RFC 4880's u = p^-1 mod q:  h = (m2 - m1) u mod q,  m = m1 + p h  (< n)
-    uint32_t q[8], uq[8], a[8], d[8], h[8];
-    const uint32_t q0inv = __ldg(&key->q0inv);
-#pragma unroll
-    for (int j = 0; j < 8; j++) { q[j] = __ldg(key->q + r * 8 + j); uq[j] = __ldg(key->uq + r * 8 + j); a[j] = m1[j]; }
-    r32::cond_sub<8, true>(a, q, r, gbase);                 // m1 < p < 2q
-    const uint32_t bt = r32::group_sub(d, m2, a, r, gbase);
-    uint32_t dq_[8];
-    r32::group_add(dq_, d, q, r, gbase);
-    r32::select_mask(d, dq_, bt);
-    mmul(h, d, uq, q, q0inv, r, gbase);
-    r32::cond_sub<8, true>(h, q, r, gbase);
-    uint32_t h16[16], m16[16], nn[16], pn[16], ph[16], mm[16];
-    widen(h, h16, r, gbase);
-    widen(m1, m16, r, gbase);
-#pragma unroll
-    for (int j = 0; j < 16; j++) { nn[j] = __ldg(key->n + r * 16 + j); pn[j] = __ldg(key->pn + r * 16 + j); }
-    mmul(ph, pn, h16, nn, __ldg(&key->n0inv), r, gbase);   // p h mod n, almost reduced
-    r32::cond_sub<16, true>(ph, nn, r, gbase);
-    r32::group_add(mm, ph, m16, r, gbase);
+    rsa_crt<BLOCK>(mm, c_lo, c_hi, key, tab, r, gbase);
     // EM = I2OSP(m, 256) into this group's shared bytes
     uint8_t* em = em_s[grp];
 #pragma unroll

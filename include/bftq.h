@@ -54,6 +54,8 @@ extern "C" {
 #define BFTQ_ERR_NO_AUTH_DATA    -17   /* crypto.ErrNoAuthenticationData (password authentication: no secret for the peer) */
 #define BFTQ_ERR_DECRYPTION_FAILED -18 /* crypto.ErrDecryptionFailed (password authentication: Zi does not open) */
 #define BFTQ_ERR_INSUFFICIENT_SECRETS -19 /* crypto.ErrInsufficientNumberOfSecrets (GetCipherKey before k secrets) */
+#define BFTQ_ERR_CERT_NOT_FOUND  -20   /* crypto.ErrCertificateNotFound: the secring is empty (Signature.Sign) */
+#define BFTQ_ERR_SIGNING_FAILED  -21   /* crypto.ErrSigningFailed: the signature failed its check against the public key */
 
 /* ---- per-item status bytes (SURVEY §8b "Errors") --------------------------------------------
  * The reference collapses every failure to ErrInvalidSignature (crypto_pgp.go:325-327); the shim
@@ -574,6 +576,27 @@ int bftq_keyring_add_private(bftq_keyring* kr, const uint8_t* packets, uint64_t 
 int bftq_message_decrypt_batch(bftq_keyring* kr, const uint8_t* raw_blob, const uint64_t* raw_off, uint64_t n_items, int32_t* out_err,
                                uint64_t* out_signed_by, uint8_t* out_flags, uint8_t* out_plain_blob, uint32_t* out_plain_len,
                                uint8_t* out_nonce_blob, uint32_t* out_nonce_len);
+
+/* ---- K12: PGPSignature.Sign / PGPCollectiveSignature.Sign (crypto_pgp.go:346-371,502-504) ----------------------------
+ * Item i signs tbs_blob[tbs_off[i] .. tbs_off[i+1]) as x/crypto's openpgp.DetachSign(w, secring[0], tbs, nil) with
+ * creation time ctime[i] (Go: time.Now()), byte for byte: the entity's primary key, SigType 0, SHA-256, creation time and
+ * issuer hashed, RSA PKCS#1 v1.5.  out_sig + i * BFTQ_SIGN_PACKET_BYTES receives the serialized signature packet
+ * (SignaturePacket.Data; Cert stays with the caller).  Its MPI header is always 08 00, as Go writes it.  The signer is the
+ * first entity registered with bftq_keyring_add(priv = 1), in replace() order; its private half must have been
+ * registered with bftq_keyring_add_private.
+ * Returned before any device work, with nothing written:
+ *   BFTQ_ERR_INVALID_ARG      NULL arguments, bad offsets
+ *   BFTQ_ERR_CERT_NOT_FOUND   the secring is empty
+ *   BFTQ_ERR_UNSUPPORTED      secring[0]'s primary key is not RSA (algo 1) with a 2048-bit modulus in the engine's key
+ *                             table, or its private half is not registered: the shim signs the batch on crypto/pgp.  This
+ *                             includes a private half dropped by bftq_keyring_remove, which drops the private halves of
+ *                             removed entities while Go's Remove leaves the secring alone.
+ *   BFTQ_ERR_NO_DEVICE        a parse-only keyring
+ * Per item: out_err[i] = 0, or BFTQ_ERR_SIGNING_FAILED when s does not verify against the public key (Go's
+ * decryptAndCheck, "rsa: internal error"); that item's packet is zeroed. */
+#define BFTQ_SIGN_PACKET_BYTES 287
+int bftq_signature_sign_batch(bftq_keyring* kr, const uint8_t* tbs_blob, const uint64_t* tbs_off, const uint32_t* ctime, uint64_t n_items,
+                              uint8_t* out_sig, int32_t* out_err);
 
 /* Batching aggregator: bftkv calls Signature.Verify one (tbs, sig) at a time from many goroutines
  * (one per peer in transport.Multicast, transport/transport.go:110-127; one per HTTP request on the
